@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """bench.py — the reference's headline metric on BASELINE.json configs[1]:
-Llama-3-8B bf16, 1xB200, batch=128 concurrent `analyze` ReAct steps over synthetic Pod YAML
+Llama-3-8B bf16, 1xH100 (80 GB), batch=128 concurrent `analyze` ReAct steps over synthetic Pod YAML
 (P=1536 prompt tokens, G=256 generated tokens, mean decode context 1664; SURVEY.md §8d config 2).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one decode forward of the whole batch (128 sequences, one new token each) through the hot path.
   value  : decode tokens/s, whole job (all N GPUs), inputs resident in HBM, K steps inside one CUDA-event bracket
@@ -12,7 +12,7 @@ A "step" is one decode forward of the whole batch (128 sequences, one new token 
            chat completions per GPU (prompt bytes in, text out), tokenisation, H2D of ids/metadata, prefill, every
            decode step's D2H of sampled ids and detokenisation inside the timed region.
   roofline: dominant kernel = paged decode attention; achieved = algorithmic KV bytes per launch / mean launch time
-           (CUDA events on the engine stream) against the measured HBM copy bandwidth.
+           (CUDA events on the engine stream) against MEASURED_PEAKS.json's HBM bandwidth if present, else the data-sheet figure.
   cpu_baseline: the CPU oracle (a port — the reference has no model arithmetic of its own) on the host cores.
 N>1 = data-parallel replicas (BASELINE configs[2]): one engine per GPU, no data-path collective, weak scaling.
 N>=2 additionally runs, AFTER the headline (metric/value unchanged), the tensor-parallel path at t = N over the same N ranks:
@@ -21,6 +21,10 @@ N>=2 additionally runs, AFTER the headline (metric/value unchanged), the tensor-
               1.08M-token prefill) at N=8, Llama-3-8B TP=2 at N=2 — decode ms/step, tokens/s per group and per GPU, fraction of the per-GPU
               HBM roofline, the all-reduce chain (in-situ us per all-reduce x count per step).
 `--impl reference` times the CPU port alone (rank 0 only), same JSON line shape.
+`--dump-outputs DIR` writes, after the timed steps, what they computed as float64 .npy files (inputs are seeded, so two builds can be
+compared output for output): decode_last_token_ids.npy = the token id each of the 128 sequences sampled in the last timed decode step,
+decode_last_token_logits.npy = those tokens' fp32 logits (the LM head fuses the arg-max, so the step never materialises other logits),
+e2e_completion_token_ids.npy = [128, 256] completion token ids of the timed end-to-end round (rank r > 0 adds the suffix _rank<r>).
 """
 import argparse
 import json
@@ -45,11 +49,11 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -360,7 +364,7 @@ def run_ours(args, rank, world, local_rank):
         torch.cuda.synchronize()
 
     # A rank that merely WAITS (while rank 0 drives every GPU in the router block) must wait on the host: an NCCL barrier is a kernel
-    # spinning on that rank's GPU, taking SMs away from the engine rank 0 runs there (measured: the served round took 8.4 s instead of 3.7 s).
+    # spinning on that rank's GPU, taking SMs away from the engine rank 0 runs there.
     cpu_group = dist.new_group(backend="gloo") if dist is not None else None
 
     def host_barrier():
@@ -413,7 +417,7 @@ def run_ours(args, rank, world, local_rank):
     # context chosen so that the mean over the K timed steps is MEAN_CTX (=P+G/2)
     ctx0 = max(64, MEAN_CTX - W - K // 2)
     # ONE sampler for the whole job (rank 0, all N GPUs): NVML queries take driver-wide locks; N polling processes are the
-    # suspected source of the host gaps seen at N=4 (0.5 ms per 8.5 ms step against 0.02 ms at N=1) and one is enough anyway
+    # possible source of host gaps in the timed steps, and one is enough anyway
     clocks = ClockSampler(",".join(str(i) for i in range(world)), 200 if world == 1 else 500) if rank == 0 else None
     if clocks:
         clocks.start()
@@ -433,14 +437,8 @@ def run_ours(args, rank, world, local_rank):
     attn_bytes = BATCH * rp["mean_ctx"] * kv_tok / L                      # K and V of every cached token, once
     peak, peak_src = measured_peaks()
     achieved = attn_bytes / (attn_launch_ms * 1e-3) / 1e9 if attn_launch_ms > 0 else 0.0
-    traffic = None
-    try:      # DRAM bytes of the same kernel from the committed `ncu --set full` capture (per launch)
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))["decode_attention_kernel<128>"]
-        traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": "decode_attention_kernel<128>", "achieved": round(achieved, 1), "peak": peak,
-                "unit": "GB/s", "frac": round(achieved / peak, 4), "traffic": traffic, "peak_source": peak_src,
+                "unit": "GB/s", "frac": round(achieved / peak, 4), "traffic": None, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": attn_bytes, "launch_ms": round(attn_launch_ms, 4),
                 "kernel_share_of_step": round(rp["attn_ms_per_step"] / rp["device_ms_per_step"], 3) if rp["device_ms_per_step"] else None,
                 "step": {"algorithmic_bytes": r["algorithmic_bytes_per_step"],
@@ -480,9 +478,16 @@ def run_ours(args, rank, world, local_rank):
     one_round()                                                                  # warm-up round
     s0 = eng.stats()
     barrier()
-    dt, _ = one_round()
+    dt, e2e_outs = one_round()
     barrier()
     s1 = eng.stats()
+    if args.dump_outputs:
+        sfx = f"_rank{rank}" if rank > 0 else ""
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"decode_last_token_ids{sfx}.npy"), np.asarray(r["last_token_ids"], dtype=np.float64))
+        np.save(os.path.join(args.dump_outputs, f"decode_last_token_logits{sfx}.npy"), np.asarray(r["last_token_logits"], dtype=np.float32))
+        np.save(os.path.join(args.dump_outputs, f"e2e_completion_token_ids{sfx}.npy"),
+                np.asarray([list(o.token_ids) for o in e2e_outs], dtype=np.float64))
     dt = allmax(dt)
     n_fwd = (s1["prefill_steps"] - s0["prefill_steps"]) + (s1["decode_steps"] - s0["decode_steps"])
     e2e = {"value": round(world * BATCH * GEN / dt, 1), "unit": "tokens/s", "react_steps_per_sec": round(world * BATCH / dt, 2),
@@ -493,6 +498,7 @@ def run_ours(args, rank, world, local_rank):
            "d2h_bytes_per_step": int((s1["d2h_bytes"] - s0["d2h_bytes"]) / max(1, n_fwd)), "forwards": n_fwd}
     launches = int(round(r["launches_per_step"] * K))
     line = {"metric": "decode_tokens_per_sec", "value": round(value, 1), "unit": "tokens/s", "n_gpus": world, "steps": K, "warmup": W,
+            "device": torch.cuda.get_device_name(local_rank),
             "ms_per_step": round(ms_step, 4), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
             "data": "synthetic (seeded random-init weights seed=1234; the reference's verbatim system prompts + seeded synthetic Pod YAML; "
                     "byte-level BPE tokenizer trained offline on OpsAgent-domain text)",
@@ -590,7 +596,7 @@ def main():
     ap.add_argument("--steps", type=int, default=64)
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--kv-gb", type=float, default=60.0, dest="kv_gb")
+    ap.add_argument("--kv-gb", type=float, default=40.0, dest="kv_gb", help="KV-cache pool per engine (80 GB HBM: 16 GB of 8B weights + 40 GB)")
     ap.add_argument("--cpu-tokens", type=int, default=24, dest="cpu_tokens")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--router-front", choices=["native", "python"], default="native", help="the serving block's front: csrc/http_server.cpp (default) or router.py + http_front.py")
@@ -607,11 +613,14 @@ def main():
     ap.add_argument("--tp-ctx", type=int, default=1024)
     ap.add_argument("--engine-extra", default="{}", dest="engine_extra", help="dev: JSON of engine options merged into the config (A/B runs)")
     ap.add_argument("--tp-deadline", type=float, default=900.0, dest="tp_deadline")
+    ap.add_argument("--dump-outputs", default="", dest="dump_outputs", metavar="DIR", help="write the timed path's outputs as .npy files into DIR")
     ap.add_argument("--tp-only", action="store_true", help="dev: only the tensor-parallel block (prints {\"tp\": ...}; NOT a bench line)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; --impl reference has no such outputs")
         run_reference(args, rank, world)
         return
     if world != args.gpus and world == 1 and args.gpus > 1:

@@ -1,5 +1,5 @@
 /*
- * opsagent_b200.h — C ABI of the B200-native local chat-completion engine.
+ * opsagent_b200.h — C ABI of the H100-native local chat-completion engine.
  *
  * This is the drop-in boundary behind OpsAgent's LLM seam.  The reference has no FFI for this path;
  * its seam is the Go method
@@ -125,7 +125,8 @@ OA_API int oa_debug_prefill_logits(oa_engine*, const int32_t* tokens, int32_t n,
  * seeded synthetic ids), then runs warmup+steps decode forwards of the whole batch, timed with CUDA events on the
  * engine stream.  out[0]=ms/step over ONE event bracket around all timed steps (host gaps included), out[1]=prefill ms, out[2]=kernel launches per step, out[3]=mean ctx over the
  * timed steps, out[4]=attention-kernel ms/step (avg), out[5]=algorithmic bytes/step,
- * out[6]=sum of per-step device durations / steps (host gaps excluded) */
+ * out[6]=sum of per-step device durations / steps (host gaps excluded); with n_out >= 8 + batch, out[8 + b] = the token id sequence b
+ * sampled in the last timed step; with n_out >= 8 + 2 * batch (single GPU), out[8 + batch + b] = that token's fp32 logit */
 OA_API int oa_bench_decode(oa_engine*, int32_t batch, int32_t ctx_len, int32_t steps, int32_t warmup, double* out, int32_t n_out);
 
 /* in-situ per-kernel-class timings accumulated while OA_PROFILE_ALL=1 (JSON name -> [total ms, launches]) */

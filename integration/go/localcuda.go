@@ -1,6 +1,6 @@
 //go:build localcuda
 
-// Package llms — `local-cuda` provider: the in-process B200 engine behind the existing Chat seam.
+// Package llms — `local-cuda` provider: the in-process H100 engine behind the existing Chat seam.
 //
 // Drop this file into the reference at pkg/llms/localcuda.go and build with
 //     CGO_ENABLED=1 go build -tags localcuda ./cmd/kube-copilot        (the reference Dockerfile:17 uses CGO_ENABLED=0)

@@ -14,10 +14,10 @@
 //   Long or ragged contexts are cut into segments by a host-made plan; partial (m, l, O) go to a workspace and
 //   decode_merge_kernel combines them (flash-decoding).
 // The 16-row mma.sync tile is the right tool here: with <= 8 real rows per tile even the legacy tensor path
-// is > 10x faster than the HBM stream it has to keep up with, and tcgen05's 128-row minimum cannot be filled.
+// has far more throughput than the HBM stream it has to keep up with, and a 64-row wgmma tile would be mostly padding.
 //
 // Prefill kernel: FlashAttention-2 style, 8 warps x 16 query rows per CTA (one TMA-fed K/V stage serves 128 query rows), same TMA ring over the paged cache
-// (new tokens' K/V are written to the cache by rope_kv_write before attention), causal mask by position.
+// (new tokens' K/V are written to the cache by rope_kv_write before attention), causal mask by position; both products on wgmma.
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -321,6 +321,9 @@ cudaError_t launch_decode_attention(const CUtensorMap* tm_kv, const KvLayout& kv
 static constexpr int PREFILL_WARPS = PREFILL_TILE_ROWS / 16;            // 8 consumer warps x 16 query rows share every K/V stage
 static constexpr int PREFILL_THREADS = (PREFILL_WARPS + 1) * 32;        // + 1 TMA producer warp
 
+// Both products on wgmma: warpgroup g (warps 4g..4g+3) owns query rows [64g, 64g + 64).  S = Q·Kᵀ is m64n64k16 with Q from registers (the mma.sync A-fragment layout) and K K-major as TMA stored it;
+// O += P·V is m64nDk16 with P from registers and V read MN-major (d contiguous, as stored).  The accumulator fragments have the
+// mma.sync C layout (register 4j + e = rows g / g+8, columns 8j + 2t + e), so the online softmax works on them directly.
 template <int D>
 __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_kv,
                                                                            const PrefillAttnParams p, const int64_t layer_row0,
@@ -389,35 +392,27 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
             qa[ks][3] = ok1 ? *reinterpret_cast<const uint32_t*>(q1 + ks * 16 + 8 + 2 * t) : 0u;
         }
     }
-    float oacc[NT][4];
+    float oacc[NT * 4];
 #pragma unroll
-    for (int j = 0; j < NT; ++j) { oacc[j][0] = oacc[j][1] = oacc[j][2] = oacc[j][3] = 0.f; }
+    for (int i = 0; i < NT * 4; ++i) oacc[i] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    const int warp_last_pos = tile.pos0 + warp * 16 + 15;      // largest query position in this warp
+    const int wg_last_pos = tile.pos0 + (warp >> 2) * 64 + 63;   // largest query position of this warpgroup: wgmma is warpgroup-wide
 
     int s = 0; uint32_t ph = 0;
     for (int c = 0; c < n_chunks; ++c) {
         mbar_wait(&full_bar[s], ph);
-        if (c * PAGE <= warp_last_pos) {
+        if (c * PAGE <= wg_last_pos) {
             const uint32_t kbase = smem_u32(smem + s * Cfg::STAGE_BYTES);
             const uint32_t vbase = kbase + Cfg::KV_BYTES;
-            float sacc[8][4];
+            float sacc[32];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { sacc[j][0] = sacc[j][1] = sacc[j][2] = sacc[j][3] = 0.f; }
-            {
-                const int rr = ((lane >> 4) << 3) + (lane & 7);
-                const int dsel = ((lane >> 3) & 1) << 3;
+            for (int i = 0; i < 32; ++i) sacc[i] = 0.f;
+            wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {           // 16 key tokens per ldmatrix.x4
-                        uint32_t b0, b1, b2, b3;
-                        ldmatrix_x4(kbase + kv_off<D>(jj * 16 + rr, ks * 16 + dsel), b0, b1, b2, b3);
-                        mma_bf16_16816(sacc[jj * 2], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b0, b1);
-                        mma_bf16_16816(sacc[jj * 2 + 1], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b2, b3);
-                    }
-                }
-            }
+            for (int ks = 0; ks < KS; ++ks)        // 16 head dims per step: +32 B inside the 128-byte row, next 64-column half at +TILE_BYTES
+                wgmma_rs_m64n64(sacc, qa[ks], gmma_desc_sw128(kbase + (uint32_t)((ks >> 2) * Cfg::TILE_BYTES + (ks & 3) * 32)), ks > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
             const bool diag = (c * PAGE + PAGE - 1) > tile.pos0 + warp * 16;   // some (row, col) pairs may be masked
             float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
@@ -425,14 +420,15 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int kpos = c * PAGE + j * 8 + 2 * t + e;
-                    float v0 = sacc[j][e] * p.scale_log2e, v1 = sacc[j][2 + e] * p.scale_log2e;
+                    float v0 = sacc[4 * j + e] * p.scale_log2e, v1 = sacc[4 * j + 2 + e] * p.scale_log2e;
                     if (diag) { if (kpos > qpos0) v0 = -INFINITY; if (kpos > qpos1) v1 = -INFINITY; }
-                    sacc[j][e] = v0; sacc[j][2 + e] = v1;
+                    sacc[4 * j + e] = v0; sacc[4 * j + 2 + e] = v1;
                     mx0 = fmaxf(mx0, v0); mx1 = fmaxf(mx1, v1);
                 }
             mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
             mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-            // chunk 0 always has key 0 <= every query position, so the running max is finite from the first chunk on
+            // chunk 0 always has key 0 <= every query position, so the running max is finite from the first chunk on; a chunk wholly
+            // in a row's future gives mx = -inf and leaves m, l and O unchanged
             const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
             const float al0 = exp2f(m0 - mn0), al1 = exp2f(m1 - mn1);
             m0 = mn0; m1 = mn1;
@@ -440,28 +436,24 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
             uint32_t pa[8][2];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const float p00 = exp2f(sacc[j][0] - mn0), p01 = exp2f(sacc[j][1] - mn0);
-                const float p10 = exp2f(sacc[j][2] - mn1), p11 = exp2f(sacc[j][3] - mn1);
+                const float p00 = exp2f(sacc[4 * j] - mn0), p01 = exp2f(sacc[4 * j + 1] - mn0);
+                const float p10 = exp2f(sacc[4 * j + 2] - mn1), p11 = exp2f(sacc[4 * j + 3] - mn1);
                 ps0 += p00 + p01; ps1 += p10 + p11;
                 pa[j][0] = pack_bf16x2(p00, p01); pa[j][1] = pack_bf16x2(p10, p11);
             }
             l0 = l0 * al0 + ps0; l1 = l1 * al1 + ps1;
 #pragma unroll
-            for (int j = 0; j < NT; ++j) { oacc[j][0] *= al0; oacc[j][1] *= al0; oacc[j][2] *= al1; oacc[j][3] *= al1; }
-            {
-                const int rr = (((lane >> 3) & 1) << 3) + (lane & 7);
-                const int dsel = (lane >> 4) << 3;
+            for (int j = 0; j < NT; ++j) { oacc[4 * j] *= al0; oacc[4 * j + 1] *= al0; oacc[4 * j + 2] *= al1; oacc[4 * j + 3] *= al1; }
+            wgmma_fence();
 #pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {               // 16 key tokens per k-step
-#pragma unroll
-                    for (int j = 0; j < NT; j += 2) {
-                        uint32_t b0, b1, b2, b3;
-                        ldmatrix_x4_trans(vbase + kv_off<D>(kk * 16 + rr, j * 8 + dsel), b0, b1, b2, b3);
-                        mma_bf16_16816(oacc[j], pa[kk * 2][0], pa[kk * 2][1], pa[kk * 2 + 1][0], pa[kk * 2 + 1][1], b0, b1);
-                        mma_bf16_16816(oacc[j + 1], pa[kk * 2][0], pa[kk * 2][1], pa[kk * 2 + 1][0], pa[kk * 2 + 1][1], b2, b3);
-                    }
-                }
+            for (int kk = 0; kk < 4; ++kk) {       // 16 key tokens per step = two 8-row groups of V (1024 B apart)
+                const uint32_t a[4] = {pa[2 * kk][0], pa[2 * kk][1], pa[2 * kk + 1][0], pa[2 * kk + 1][1]};
+                const uint64_t db = gmma_desc_sw128_mn(vbase + (uint32_t)(kk * 2048), (uint32_t)Cfg::TILE_BYTES, 1024u);
+                if constexpr (D == 128) wgmma_rs_m64n128_tb(oacc, a, db, 1u);
+                else wgmma_rs_m64n64_tb(oacc, a, db, 1u);
             }
+            wgmma_commit();
+            wgmma_wait<0>();                        // V of this stage has been read
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[s]);
@@ -475,12 +467,12 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
     if (r0 < tile.n_rows) {
         uint16_t* o = ob + (size_t)(tile.q_row0 + r0) * ldo;
 #pragma unroll
-        for (int j = 0; j < NT; ++j) *reinterpret_cast<uint32_t*>(o + j * 8 + 2 * t) = pack_bf16x2(oacc[j][0] * inv0, oacc[j][1] * inv0);
+        for (int j = 0; j < NT; ++j) *reinterpret_cast<uint32_t*>(o + j * 8 + 2 * t) = pack_bf16x2(oacc[4 * j] * inv0, oacc[4 * j + 1] * inv0);
     }
     if (r1 < tile.n_rows) {
         uint16_t* o = ob + (size_t)(tile.q_row0 + r1) * ldo;
 #pragma unroll
-        for (int j = 0; j < NT; ++j) *reinterpret_cast<uint32_t*>(o + j * 8 + 2 * t) = pack_bf16x2(oacc[j][2] * inv1, oacc[j][3] * inv1);
+        for (int j = 0; j < NT; ++j) *reinterpret_cast<uint32_t*>(o + j * 8 + 2 * t) = pack_bf16x2(oacc[4 * j + 2] * inv1, oacc[4 * j + 3] * inv1);
     }
 }
 

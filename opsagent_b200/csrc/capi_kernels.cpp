@@ -107,7 +107,7 @@ int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t
     cudaError_t e;
     if (decode) {
         DecodePlan plan;
-        build_decode_plan(ctx_lens, n_seqs, n_kv, 2 * 148, force_splits, plan);
+        build_decode_plan(ctx_lens, n_seqs, n_kv, 2 * 132, force_splits, plan);
         DevBuf d_segs(plan.segs.size() * sizeof(DecodeSeg)), d_ptr(plan.cta_ptr.size() * 4), d_merge(plan.merges.size() * sizeof(MergeItem));
         DevBuf d_po((size_t)(plan.n_slots + 1) * grp * head_dim * 4), d_pml((size_t)(plan.n_slots + 1) * grp * 2 * 4);
         if (!d_segs.p || !d_ptr.p || !d_merge.p || !d_po.p || !d_pml.p) return OA_ERR_INTERNAL;
@@ -134,13 +134,7 @@ int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t
     cudaMemcpyAsync(d_tiles.p, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, s);
     PrefillAttnParams a{}; a.q = q; a.out = out; a.block_tables = (const int32_t*)d_bt.p; a.max_pages_per_seq = max_pages_per_seq;
     a.tiles = (const PrefillTile*)d_tiles.p; a.n_tiles = (int)tiles.size(); a.layer = 0; a.n_heads = n_heads; a.n_kv = n_kv; a.scale_log2e = scale_log2e;
-    const char* leg = std::getenv("OA_PREFILL_ATTN");
-    if (leg && std::string(leg) == "legacy") e = launch_prefill_attention(&tm, kv, a, s);
-    else {
-        CUtensorMap tmq;
-        if (make_tmap_bf16_2d(&tmq, q, (uint64_t)total_q, (uint64_t)n_heads * head_dim, (uint64_t)n_heads * head_dim, 128, 64) != 0) return OA_ERR_INTERNAL;
-        e = launch_prefill_attention_tc(&tmq, &tm, kv, a, s);
-    }
+    e = launch_prefill_attention(&tm, kv, a, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     return rc_of(e);
 }

@@ -1,4 +1,4 @@
-// common.cuh — device-side building blocks for sm_100a: bf16 helpers, mbarrier, TMA, tcgen05/TMEM,
+// common.cuh — device-side building blocks for sm_90a: bf16 helpers, mbarrier, TMA, wgmma,
 // ldmatrix/mma.sync wrappers.  Everything here is inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda_bf16.h>
@@ -127,91 +127,148 @@ OA_DEVINL void tma_prefetch_l2_2d(const void* tmap, int32_t c0, int32_t c1) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (Hopper warpgroup MMA): D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, bf16 operands K-major in shared memory, fp32
+// accumulators in the registers of the issuing warpgroup (4 aligned warps, 128 threads, all of which execute every call).
+// Fragment of m64nN: register r of thread (warp w of the warpgroup, lane l) holds
+//   row = 16w + l/4 + 8*((r >> 1) & 1),  col = 8*(r >> 2) + 2*(l & 3) + (r & 1).
 // ---------------------------------------------------------------------------------------------
-OA_DEVINL void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-OA_DEVINL void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// whole warp; writes the TMEM base address to *smem_dst
-template <uint32_t kCols>
-OA_DEVINL void tmem_alloc(uint32_t* smem_dst) {
-    static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(kCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-OA_DEVINL void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulation
-OA_DEVINL void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-OA_DEVINL void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp receives lane (base_lane + i), columns c..c+31
-OA_DEVINL void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-// registers -> TMEM, same 32 lanes x 32 columns shape
-OA_DEVINL void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-          "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-          "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-          "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-OA_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-OA_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+OA_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+OA_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+OA_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// UMMA shared-memory matrix descriptor, K-major operand tile stored as rows of 128 B with the
-// 128-byte swizzle (what a TMA box {64 bf16, rows} with CU_TENSOR_MAP_SWIZZLE_128B produces):
-//   start address >>4 in [0,14); LBO (unused for swizzled K-major, set to 1) in [16,30);
-//   SBO = 1024 B (8 rows x 128 B) >>4 in [32,46); version = 1 in [46,48); layout SWIZZLE_128B = 2 in [61,64).
-OA_DEVINL uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor of a K-major operand tile stored as rows of 128 B with the 128-byte swizzle (what a TMA box
+// {64 bf16, rows} with CU_TENSOR_MAP_SWIZZLE_128B produces): start address >>4 in [0,14); LBO (unused for swizzled K-major) = 1
+// in [16,30); SBO = 1024 B (8 rows x 128 B) >>4 in [32,46); layout SWIZZLE_128B = 1 in [62,64).  Stepping 16 bf16 (32 B) along K
+// inside the swizzle row is +2 in the address field.
+OA_DEVINL uint64_t gmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// MN-major B operand (e.g. V[kv, d] with d contiguous used as B[N = d, K = kv]): 128-byte swizzled atoms of 64 N-elements x 8
-// K-rows (1024 B); SBO = byte stride between consecutive 8-row K groups, LBO = byte stride between 64-element N blocks.
-OA_DEVINL uint64_t umma_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+
+#define OA_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define OA_F16(i) OA_F4(i), OA_F4(i + 4), OA_F4(i + 8), OA_F4(i + 12)
+OA_DEVINL void wgmma_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : OA_F16(0)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : OA_F16(0), OA_F16(16)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : OA_F16(0), OA_F16(16), OA_F16(32), OA_F16(48)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+// MN-major operand (e.g. V[kv, d] with d contiguous used as B[N = d, K = kv]), 128-byte swizzle: atoms of 64 N-elements x 8 K-rows
+// (1024 B); LBO = byte stride between 64-element N blocks, SBO = byte stride between 8-row K groups.
+OA_DEVINL uint64_t gmma_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_bmn(uint32_t m, uint32_t n) {      // as umma_idesc_bf16 with B MN-major (bit 16)
-    return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
+// A from registers (4 x bf16x2 per thread, the mma.sync m16n8k16 A-fragment layout for the warp's 16 rows); *_tb: B MN-major
+OA_DEVINL void wgmma_rs_m64n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : OA_F16(0), OA_F16(16)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc) : "memory");
 }
-// instruction descriptor: D fp32 (bits 4-5 = 1), A/B bf16 (bits 7-9, 10-12 = 1), both K-major,
-// N>>3 in [17,23), M>>4 in [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
+OA_DEVINL void wgmma_rs_m64n64_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+        : OA_F16(0), OA_F16(16)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_rs_m64n128_tb(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+        : OA_F16(0), OA_F16(16), OA_F16(32), OA_F16(48)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc) : "memory");
+}
+template <int N>
+OA_DEVINL void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+    if constexpr (N == 32) wgmma_m64n32(d, da, db, acc);
+    else if constexpr (N == 64) wgmma_m64n64(d, da, db, acc);
+    else { static_assert(N == 128, "wgmma N in {32, 64, 128}"); wgmma_m64n128(d, da, db, acc); }
+}
+
+// fp32 accumulator tile [rows][N] in shared memory, 16-byte chunks XOR-swizzled by (row & 7): a warp storing its wgmma fragment
+// and a warp reading 32 consecutive columns of 32 rows (one row per lane) are both free of bank conflicts.  N >= 32.
+OA_DEVINL int acc_idx(int N, int row, int col) { return row * N + ((((col >> 2) ^ row) & 7) | ((col >> 2) & ~7)) * 4 + (col & 3); }
+// warpgroup fragment of rows [row0, row0 + 64) -> the shared tile
+template <int N>
+OA_DEVINL void acc_store_frag(float* acc, int row0, const float (&d)[N / 2]) {
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 16 * w + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc + acc_idx(N, row, col)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+        }
+    }
+}
+OA_DEVINL float4 acc_ld4(const float* acc, int N, int row, int col) { return *reinterpret_cast<const float4*>(acc + acc_idx(N, row, col)); }
+// one row x 32 columns [col0, col0 + 32) (col0 % 32 == 0) as raw fp32 bits
+OA_DEVINL void acc_ld32(const float* acc, int N, int row, int col0, uint32_t (&v)[32]) {
+#pragma unroll
+    for (int c = 0; c < 32; c += 4) {
+        const float4 x = acc_ld4(acc, N, row, col0 + c);
+        v[c] = __float_as_uint(x.x); v[c + 1] = __float_as_uint(x.y); v[c + 2] = __float_as_uint(x.z); v[c + 3] = __float_as_uint(x.w);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -98,14 +98,14 @@ struct EngineOptions {
     int bn_qkv = 0, bn_o = 0, bn_gu = 0, bn_down = 0, bn_lm = 0;   // GEMM N-tile overrides (0 = heuristic)
     int attn_ctas = 0;            // decode attention CTA count override (0 = 2 per SM)
     int streamk = 1;              // decode (T <= 128) projections through the persistent stream-K GEMM
-    int sk_bn = 128, sk_ctas = 0; // its N tile (128: half the partial traffic, measured faster than 256) and CTA count (0 = one per SM)
-    int sk_max_rows = 128;        // batches up to this many rows use stream-K (256 = two row tiles: measured SLOWER than the tile GEMM on Qwen-32B TP=4 B=256: 22.2 vs 18.5 ms)
-    int sk_fuse_swiglu = 1;       // gate/up projection: the CTA holding a tile's first k-block adds the other pieces and writes silu(gate)*up from TMEM (no SwiGLU kernel)
+    int sk_bn = 128, sk_ctas = 0; // its N tile (128: half the partial traffic of 256, and a 64 x 128 fp32 fragment per consumer warpgroup) and CTA count (0 = one per SM)
+    int sk_max_rows = 128;        // batches up to this many rows use stream-K (256 = two row tiles, opt-in)
+    int sk_fuse_swiglu = 1;       // gate/up projection: the CTA holding a tile's first k-block adds the other pieces and writes silu(gate)*up from its accumulator (no SwiGLU kernel)
     int sk_fuse_epi = 0;          // bitmask — 1: qkv finishes bias + RoPE + paged-KV write, 2: o, 4: down finish the residual add inside the stream-K GEMM (the CTA holding a tile's first k-block; a norm-only kernel follows o / down).
-                                  // Bit-identical to the consumers; default set from the measured sweep (profiles/r02_*): few tiles cut into 4-5 pieces each make the finishers a serial tail
+                                  // Bit-identical to the consumers; off by default: few tiles cut into 4-5 pieces each make the finishers a serial tail
     int sk_clusterk = 0;          // bitmask — 1: qkv, 2: o, 4: down as a cluster split-K GEMM with DSMEM reduction and the epilogue (RoPE + KV write / residual) inside (gemm_clusterk.cu), where the shape fills >= 80 % of the SMs
     int sk_clusterk_min_fill = 80; // ... and only where n_tiles x cluster size covers at least this percentage of the SMs (tests: 0)
-    int sk_l2_prefetch_kb = 0;    // per-CTA weight KB prefetched into L2 ahead of the dependency wait (measured: hurts, 8.75 -> 9.3 ms; off)
+    int sk_l2_prefetch_kb = 0;    // per-CTA weight KB prefetched into L2 ahead of the dependency wait (0 = off)
     int sk_bn_qkv = 0, sk_bn_o = 0, sk_bn_gu = 0, sk_bn_down = 0;   // per-projection overrides (0 = sk_bn)
     int start_thread = 1;
     std::string model_aliases;    // other model names this engine answers to, comma separated ("*" = any): the reference sends currentModel or "gpt-4" (execute.go:168-171)
@@ -116,13 +116,12 @@ struct EngineOptions {
     int prefill_batch_tokens = 2048;   // while sequences are decoding, new requests wait until this many uncached prompt tokens are queued ...
     int prefill_max_wait_ms = 20;      // ... or the oldest has waited this long: one weight pass then prefills several arrivals (0 tokens = admit at once)
     int mixed_steps = 1;               // decoding sequences ride along in prefill steps (decode attention for their rows, prefill attention for the chunks) instead of stalling for every arrival's weight pass; 0 = prefill-first steps only
-                                       // (react loop with 100 ms tool latency: 95.7 vs 92.1 steps/s, profiles/r02e_react_mixed_ab.md)
     int react_tool_steps = 3;     // json_mode: conversations with fewer assistant turns than this get a tool call, later ones a final answer
     int tp = 1, tp_rank = 0;      // tensor parallel degree / this process's rank (one process per GPU)
     std::string tp_shm = "/oa_tp"; // POSIX shm name shared by the ranks of one TP group
     int tp_ar_bf16 = 1;            // decode all-reduce on bf16 partials (half the NVLink bytes; the prefill path always exchanged bf16); 0 = fp32 partials
     int tp_nvls = 0;               // 1: decode all-reduce inside the NVLink switch (multimem.ld_reduce / multimem.st on a multicast buffer, tp_nvls.cpp) when every rank can set it up.  Built, parity-green,
-                                   // measured SLOWER than the peer-memory one-shot at decode sizes (t=2: 38.6-43.2 vs 25.1 us per all-reduce: three dependent cross-GPU latencies instead of one; profiles/r02g_nvls.md): opt-in
+                                   // opt-in: three dependent cross-GPU latencies on the critical path instead of the peer-memory one-shot's one
     int tp_two_shot_rows = 1024;   // prefill chunks of at least this many rows use the two-shot all-reduce (reduce-scatter + all-gather: 2(t-1)/t instead of (t-1) partials' bytes per rank); smaller ones the one-shot
     uint64_t tp_nonce = 0;         // per-launch id shared by the ranks (e.g. the rendezvous port + a timestamp): followers ignore segments of other launches (0 = not checked)
 };

@@ -269,6 +269,13 @@ public:
             // SURVEY.md §8d: W_dec + sum ctx*KVB + B*KVB (the new token's KV write)
             out[5] = (model_.cfg.decode_weight_bytes() + (double)batch * mean_ctx * (double)model_.cfg.kv_bytes_per_token() +
                       (double)batch * (double)model_.cfg.kv_bytes_per_token()) / opt_.tp;      // per GPU (SURVEY §8d: W_dec/t + ctx*KVB/t)
+            if (n_out >= 8 + batch)                 // the token ids the last timed step sampled, one per sequence
+                for (int b = 0; b < batch; ++b) out[8 + b] = (double)last[b];
+            if (n_out >= 8 + 2 * batch && opt_.tp == 1) {   // ... and their fp32 logits
+                std::vector<float> top(batch);
+                model_.sampled_logits(batch, top.data());
+                for (int b = 0; b < batch; ++b) out[8 + batch + b] = (double)top[b];
+            }
         } catch (const std::exception& ex) { return fail(OA_ERR_INTERNAL, ex.what()); }
         return OA_OK;
     }
@@ -831,6 +838,6 @@ int oa_host_bpe_decode(const char* tokenizer_json_path, const int32_t* ids, int3
 
 int oa_engine_serve(oa_engine* h) { if (!h) return fail(OA_ERR_BAD_REQUEST, "null engine"); return h->e->serve(); }
 uint64_t oa_kernel_launches(void) { return launches_total(); }
-const char* oa_version(void) { return "opsagent_b200 0.1 (sm_100a)"; }
+const char* oa_version(void) { return "opsagent_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

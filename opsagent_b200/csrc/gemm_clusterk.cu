@@ -1,14 +1,14 @@
-// gemm_clusterk.cu — decode projections with FEW output tiles (o, down, qkv: 32-48 tiles of 128 columns on 148 SMs) as a
+// gemm_clusterk.cu — decode projections with FEW output tiles (o, down, qkv: 32-48 tiles of 128 columns on 132 SMs) as a
 // cluster split-K GEMM: the S CTAs of one thread-block cluster own ONE 128 x 128 output tile and a 1/S slice of K each, reduce their
-// TMEM accumulators through distributed shared memory and finish the epilogue together — no fp32 partial round trip through L2, no
-// consumer launch, no serial tail of a few finishing CTAs (what made the stream-K finisher fusion slower, profiles/r02a).
+// register accumulators through distributed shared memory and finish the epilogue together — no fp32 partial round trip through L2, no
+// consumer launch, no serial tail of a few finishing CTAs (the weakness of the stream-K finisher fusion on these shapes).
 //
 //   grid = n_tiles x S CTAs, cluster (S,1,1); CTA (tile, r) streams k-blocks [r*kb/S, (r+1)*kb/S) of the tile's weights
-//   warp 0   : TMA producer (weights issued BEFORE griddepcontrol.wait: they depend on no predecessor)
-//   warp 1   : tcgen05.mma 128 x 128 x 16 into TMEM
-//   warps 2-5: TMEM -> registers -> st.shared::cluster into the OWNER CTA of each 32 x 64 "pair unit" (8 per tile, owner = unit % S);
+//   warp 8   : TMA producer (weights issued BEFORE griddepcontrol.wait: they depend on no predecessor)
+//   warps 0-7: two warpgroups, wgmma 64 x 128 x 16 each (rows [64g, 64g + 64)) into registers, then st.shared::cluster of the fragments
+//              into the OWNER CTA of each 32 x 64 "pair unit" (8 per tile, owner = unit % S);
 //              after one cluster barrier every CTA sums the S partials of its own units IN RANK ORDER (deterministic) and applies the
-//              epilogue with all 128 threads: residual add into the bf16 stream (o / down) or bias + RoPE + paged-KV write (qkv).
+//              epilogue with warps 0-3: residual add into the bf16 stream (o / down) or bias + RoPE + paged-KV write (qkv).
 // A pair unit = rows [32q, 32q+32) x the two 32-column chunks that RoPE rotates together (columns i and i + D/2 of one head), so every
 // epilogue is thread-local.  The K split differs from the stream-K path, so results are equal to it only up to fp32 summation order
 // (parity against the oracle holds with the same tolerance; the bit-identity test covers the stream-K variants among themselves).
@@ -19,7 +19,8 @@
 
 namespace oa {
 
-static constexpr int CK_BM = 128, CK_BN = 128, CK_BK = 64, CK_THREADS = 192, CK_STAGES = 4;
+static constexpr int CK_BM = 128, CK_BN = 128, CK_BK = 64, CK_STAGES = 4;
+static constexpr int CK_CONSUMER_WARPS = 8, CK_THREADS = 32 * (CK_CONSUMER_WARPS + 1);
 static constexpr int CK_A_BYTES = CK_BM * CK_BK * 2, CK_B_BYTES = CK_BN * CK_BK * 2, CK_STAGE_BYTES = CK_A_BYTES + CK_B_BYTES;
 static constexpr int CK_ROW_F = 36;                              // 32 + 4 pad floats: conflict-free 16-byte accesses
 static constexpr int CK_BUF_F = 32 * CK_ROW_F;                   // one 32 x 32 partial chunk
@@ -32,8 +33,8 @@ struct CkEpi {
 
 OA_DEVINL uint32_t ck_cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 OA_DEVINL uint32_t ck_mapa(uint32_t addr, uint32_t rank) { uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r; }
-OA_DEVINL void ck_st_cluster_f4(uint32_t addr, float a, float b, float c, float d) {
-    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+OA_DEVINL void ck_st_cluster_f2(uint32_t addr, float a, float b) {
+    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 OA_DEVINL void ck_cluster_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -51,8 +52,6 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
     float* recv = reinterpret_cast<float*>(smem + CK_STAGES * CK_STAGE_BYTES);          // [SLOTS][2 members][S partials][32][36]
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(recv + SLOTS * 2 * S * CK_BUF_F);
     uint64_t* empty_bar = full_bar + CK_STAGES;
-    uint64_t* acc_bar = empty_bar + CK_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t rank = ck_cluster_rank();
@@ -60,20 +59,16 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
     const int kb_total = (K + CK_BK - 1) / CK_BK;
     const int kb0 = (int)((long long)rank * kb_total / S), kb1 = (int)((long long)(rank + 1) * kb_total / S), n_kb = kb1 - kb0;   // host: kb_total >= S
 
-    if (warp == 0 && lane == 0) {
+    if (warp == CK_CONSUMER_WARPS && lane == 0) {
         tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-        for (int s = 0; s < CK_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(acc_bar, 1);
+        for (int s = 0; s < CK_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CK_CONSUMER_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<128>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_launch();
 
-    if (warp == 0) {
+    float d[CK_BN / 2] = {};
+    if (warp == CK_CONSUMER_WARPS) {
         if (lane == 0) {
             const int pre = n_kb < CK_STAGES ? n_kb : CK_STAGES;
             for (int i = 0; i < pre; ++i) {          // weights first: the HBM stream starts while the predecessor drains
@@ -92,49 +87,46 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
                 if (++s == CK_STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_bf16(CK_BM, CK_BN);
-            int s = 0; uint32_t ph = 0;
-            for (int i = 0; i < n_kb; ++i) {
-                mbar_wait(&full_bar[s], ph);
-                tcgen05_fence_after();
-                const uint32_t a_addr = smem_u32(smem + s * CK_STAGE_BYTES);
-                const uint64_t a_desc = umma_desc_sw128(a_addr), b_desc = umma_desc_sw128(a_addr + CK_A_BYTES);
+    } else if (warp < CK_CONSUMER_WARPS) {
+        const int g = warp >> 2;
+        int s = 0; uint32_t ph = 0, prev = ~0u;
+        for (int i = 0; i < n_kb; ++i) {
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t st = smem_u32(smem + s * CK_STAGE_BYTES);
+            const uint64_t da = gmma_desc_sw128(st + (uint32_t)(g * 64 * 128)), db = gmma_desc_sw128(st + CK_A_BYTES);
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < CK_BK / 16; ++k) umma_bf16(tmem_base, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc, (i | k) != 0);
-                umma_commit(&empty_bar[s]);
-                if (++s == CK_STAGES) { s = 0; ph ^= 1; }
-            }
-            umma_commit(acc_bar);
+            for (int k = 0; k < CK_BK / 16; ++k) wgmma_bf16<CK_BN>(d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (i | k) != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();                                      // one group in flight; the previous slot is free
+            if (prev != ~0u && lane == 0) mbar_arrive(&empty_bar[prev]);
+            prev = (uint32_t)s;
+            if (++s == CK_STAGES) { s = 0; ph ^= 1; }
         }
+        wgmma_wait<0>();
     }
     // every CTA of the cluster is running (co-scheduled) and past its setup before anybody writes into a peer's shared memory
     ck_cluster_sync();
-    if (warp >= 2) {
-        const int q = warp & 3;                                   // TMEM lanes / tile rows [32q, 32q + 32)
+    if (warp < CK_CONSUMER_WARPS) {
+        // fragment (row, col pair) -> the pair unit that owns it, in the owner CTA's receive buffer
         griddep_wait();
-        mbar_wait(acc_bar, 0);
-        tcgen05_fence_after();
+        const int g = warp >> 2, w = warp & 3;
         const uint32_t recv_base = smem_u32(recv);
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-            tmem_ld_wait();
-            int pidx, member; ck_pair_of<D>(c, pidx, member);
-            const int pu = q * 2 + pidx, owner = pu % S, slot = pu / S;
-            const uint32_t local = recv_base + (uint32_t)((((slot * 2 + member) * S + (int)rank) * CK_BUF_F + lane * CK_ROW_F) * 4);
-            const uint32_t remote = ck_mapa(local, (uint32_t)owner);
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                ck_st_cluster_f4(remote + (uint32_t)(j * 4), __uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+        for (int j = 0; j < CK_BN / 8; ++j) {
+            int pidx, member; ck_pair_of<D>(j >> 2, pidx, member);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = g * 64 + 16 * w + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
+                const int pu = (row >> 5) * 2 + pidx, owner = pu % S, slot = pu / S;
+                const uint32_t local = recv_base + (uint32_t)((((slot * 2 + member) * S + (int)rank) * CK_BUF_F + (row & 31) * CK_ROW_F + (col & 31)) * 4);
+                ck_st_cluster_f2(ck_mapa(local, (uint32_t)owner), d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+            }
         }
-        tcgen05_fence_before();
     }
     ck_cluster_sync();                                            // all partials of my units have landed in my shared memory
-    if (warp >= 2) {
-        const int t = (int)threadIdx.x - 64;                      // 0..127
+    if (warp < 4) {
+        const int t = (int)threadIdx.x;                           // 0..127
         const int r32 = t >> 2, col8 = (t & 3) * 8;
 #pragma unroll 1
         for (int slot = 0; slot < SLOTS; ++slot) {
@@ -208,9 +200,6 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
             }
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) { tcgen05_fence_after(); tmem_dealloc<128>(tmem_base); }
 }
 
 template <int S>

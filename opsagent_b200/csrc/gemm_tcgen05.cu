@@ -1,12 +1,13 @@
-// gemm_tcgen05.cu — C[M,N] = A[M,K] · B[N,K]^T for the QKV / O / gate-up / down / LM-head projections.
+// gemm_tcgen05.cu — C[M,N] = A[M,K] · B[N,K]^T for the QKV / O / gate-up / down / LM-head projections (the file keeps its
+// name from the Blackwell version; everything in it is Hopper wgmma).
 //
-// sm_100a design (one CTA = one 128 x BLOCK_N output tile):
-//   warp 0   : TMA producer — cp.async.bulk.tensor 2D boxes {64 x 128} of A and {64 x BLOCK_N} of B into a
-//              STAGES-deep shared-memory ring (128-byte swizzle), completion on `full` mbarriers.
-//   warp 1   : allocates TMEM and issues tcgen05.mma (UMMA 128 x BLOCK_N x 16, bf16 -> fp32 in TMEM) from a
-//              single thread; tcgen05.commit releases ring slots (`empty`) and finally signals `acc_full`.
-//   warps 2-5: epilogue — tcgen05.ld the accumulator (thread = one output row, 32 columns per load), apply the
-//              fused epilogue (bias | residual add | SwiGLU | fp32 logits + row arg-max) and store.
+// sm_90a design (one CTA = one 128 x BLOCK_N output tile):
+//   warp 8    : TMA producer — cp.async.bulk.tensor 2D boxes {64 x 128} of A and {64 x BLOCK_N} of B into a
+//               STAGES-deep shared-memory ring (128-byte swizzle), completion on `full` mbarriers.
+//   warps 0-7 : two consumer warpgroups; warpgroup g issues wgmma 64 x BLOCK_N x 16 (bf16 -> fp32 in registers) for rows
+//               [64g, 64g + 64) of the tile, releases ring slots (`empty`) as their MMAs retire, and at the end of a tile
+//               writes the accumulator into a swizzled fp32 tile in shared memory (`acc_full`).
+//   epilogue  : then warpgroup 0, one output row per thread (bias | residual add | SwiGLU | fp32 logits + row arg-max).
 // Decode (M <= 128) is weight-streaming and HBM-bound: B tiles are fetched with an evict-first L2 policy, the
 // small A operand with evict-last.  K tails and M/N tails rely on TMA zero fill + predicated stores.
 //
@@ -24,33 +25,84 @@ namespace oa {
 
 static constexpr int BLOCK_M = 128;
 static constexpr int BLOCK_K = 64;     // 64 bf16 = 128 B = one swizzle row
-static constexpr int UMMA_K = 16;
-static constexpr int GEMM_THREADS = 192;
+static constexpr int EPI_WARP0 = 0, PRODUCER_WARP = 8;
+// 2 consumer warpgroups + 1 producer warp: 9 warps leave 168 registers per thread, room for a 64 x 256 fp32 fragment (128)
+static constexpr int GEMM_THREADS = 32 * (PRODUCER_WARP + 1);
+#define OA_GEMM_REGS __launch_bounds__(GEMM_THREADS, 1)
 static constexpr int RASTER_GROUP_M = 16;
+static constexpr int SMEM_LIMIT = 232448;                           // opt-in shared memory of one CTA on sm_90
+
+// Consumer side of the ring: n_kb k-blocks into this warpgroup's registers (rows [64g, 64g + 64) of each of the MT 128-row A tiles).
+// One wgmma group stays in flight; a slot is released (one arrival per consumer warp) once the group that read it has retired.
+template <int BN, int MT, int STAGES, int STAGE_BYTES, int A_TILE_BYTES, int A_BYTES>
+OA_DEVINL void wg_mma_run(float (&d)[MT][BN / 2], uint8_t* smem, uint64_t* full_bar, int& s, uint32_t& ph, int n_kb) {
+    uint64_t* empty_bar = full_bar + STAGES;
+    const uint32_t g_off = (threadIdx.x >> 7) * 64 * 128;
+    const bool leader = (threadIdx.x & 31) == 0;
+    int prev = -1;
+    for (int i = 0; i < n_kb; ++i) {
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t st = smem_u32(smem) + (uint32_t)(s * STAGE_BYTES);
+        const uint64_t db = gmma_desc_sw128(st + (uint32_t)A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int m = 0; m < MT; ++m) {
+            const uint64_t da = gmma_desc_sw128(st + (uint32_t)(m * A_TILE_BYTES) + g_off);
+            // a 256-wide tile is issued as two 128-wide halves: the m64n256 fragment is the two m64n128 fragments side by side, and
+            // one instruction with 128 live accumulators does not fit the register budget
+            constexpr int NW = BN > 128 ? 128 : BN;
+#pragma unroll
+            for (int nb = 0; nb < BN / NW; ++nb) {
+                float (&dh)[NW / 2] = *reinterpret_cast<float (*)[NW / 2]>(&d[m][nb * (NW / 2)]);
+#pragma unroll
+                for (int k = 0; k < BLOCK_K / 16; ++k)
+                    wgmma_bf16<NW>(dh, da + (uint64_t)(k * 2), db + (uint64_t)(nb * NW * 8 + k * 2), (i > 0 || k > 0) ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+}
+// registers -> the shared accumulator tile [MT * 128][BN], then one arrival per consumer warp on `bar`
+template <int BN, int MT>
+OA_DEVINL void wg_acc_publish(float* acc, const float (&d)[MT][BN / 2], uint64_t* bar) {
+    const int g = threadIdx.x >> 7;
+#pragma unroll
+    for (int m = 0; m < MT; ++m) acc_store_frag<BN>(acc, m * BLOCK_M + g * 64, d[m]);
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+constexpr int CONSUMER_WARPS = 8;
 
 template <int BN>
 struct GemmCfg {
     static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;              // 16 KB
     static constexpr int B_BYTES = BN * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    // fill ~200 KB / (CTAs per SM we want): small tiles keep several CTAs resident
-    static constexpr int STAGES = BN >= 256 ? 4 : (BN >= 128 ? 6 : (BN >= 64 ? 4 : 4));
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-    static constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
+    static constexpr int ACC_BYTES = BLOCK_M * BN * 4;
+    // the fp32 accumulator tile shares the 227 KB with the ring; one CTA per SM at every width (288 threads x 168 registers)
+    static constexpr int STAGES = BN >= 256 ? 2 : 4;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget of one CTA");
 };
 
 template <int BN, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS) gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA,
+__global__ void OA_GEMM_REGS gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                       const __grid_constant__ CUtensorMap tmB,
                                                                       const GemmParams p) {
     using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    float* acc = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::ACC_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* acc_bar = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -67,22 +119,18 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tcgen05_kernel(const __grid
     }
     const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(acc_bar, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
+        mbar_init(acc_bar, CONSUMER_WARPS);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_launch();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= PRODUCER_WARP) {
+        if (warp == PRODUCER_WARP && lane == 0) {
             // weights (B) are written by no kernel of the chain: fill the ring with them BEFORE waiting for the predecessor
             const int pre = num_kb < STAGES ? num_kb : STAGES;
             for (int kb = 0; kb < pre; ++kb) {
@@ -103,42 +151,25 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tcgen05_kernel(const __grid
                 if (++s == STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BLOCK_M, BN);
-            int s = 0; uint32_t ph = 0;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full_bar[s], ph);
-                tcgen05_fence_after();
-                const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                const uint64_t a_desc = umma_desc_sw128(a_addr);
-                const uint64_t b_desc = umma_desc_sw128(a_addr + Cfg::A_BYTES);
-#pragma unroll
-                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                    // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in the (>>4) address field
-                    umma_bf16(tmem_base, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-                }
-                umma_commit(&empty_bar[s]);   // slot reusable once these MMAs have read it
-                if (++s == STAGES) { s = 0; ph ^= 1; }
-            }
-            umma_commit(acc_bar);             // accumulator complete
-        }
-    } else {
-        // ---------------- epilogue: warps 2..5, TMEM lane group = warp % 4 ----------------
+    } else if (warp < CONSUMER_WARPS) {
+        float d[1][BN / 2] = {};
+        int s = 0; uint32_t ph = 0;
+        wg_mma_run<BN, 1, STAGES, Cfg::STAGE_BYTES, Cfg::A_BYTES, Cfg::A_BYTES>(d, smem, full_bar, s, ph, num_kb);
+        wg_acc_publish<BN, 1>(acc, d, acc_bar);
+        if (warp >= 4) return;
+        // ---------------- epilogue: warpgroup 0, rows [32q, 32q + 32) with q = warp % 4 ----------------
         const int q = warp & 3;
         const int row = m_blk * BLOCK_M + q * 32 + lane;
         const bool row_ok = row < p.M;
         griddep_wait();                   // bias/residual reads and every store below come after the predecessor grid
         mbar_wait(acc_bar, 0);
-        tcgen05_fence_after();
         float best_v = -INFINITY; int best_i = 0x7fffffff;
         const uint32_t* mask_row = nullptr;
         if (EPI == EPI_LOGITS && row_ok && p.mask_slot) { const int ms = p.mask_slot[row]; if (ms >= 0) mask_row = p.mask_table + (size_t)ms * p.mask_words; }
 #pragma unroll 1
         for (int c = 0; c < BN; c += 32) {
             uint32_t v[32];
-            tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-            tmem_ld_wait();
+            acc_ld32(acc, BN, q * 32 + lane, c, v);
             const int col0 = n_blk * BN + c;
             if (EPI == EPI_STORE) {
                 if (row_ok) {
@@ -233,12 +264,6 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tcgen05_kernel(const __grid
             p.amax_val[(size_t)row * n_tiles + n_blk] = best_v;
             p.amax_idx[(size_t)row * n_tiles + n_blk] = best_i;
         }
-        tcgen05_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
     }
 }
 
@@ -247,7 +272,7 @@ int gemm_n_tiles(int N, int block_n) { return (N + block_n - 1) / block_n; }
 template <int BN, int EPI>
 static cudaError_t launch_one(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, cudaStream_t stream) {
     using Cfg = GemmCfg<BN>;
-    auto kern = gemm_tcgen05_kernel<BN, EPI>;
+    auto kern = gemm_wgmma_kernel<BN, EPI>;
     static bool attr_done[16] = {};
     { cudaError_t e = ensure_dynamic_smem(kern, Cfg::SMEM_BYTES, attr_done); if (e != cudaSuccess) return e; }
     dim3 grid(((p.N + BN - 1) / BN) * ((p.M + BLOCK_M - 1) / BLOCK_M), 1, 1);
@@ -266,6 +291,7 @@ static cudaError_t launch_bn(const CUtensorMap* tmA, const CUtensorMap* tmB, con
 }
 
 static bool persistent_disabled();
+static constexpr int PERSIST_BN = 128;      // 64 accumulator registers per consumer thread: no spills, and a 4-deep ring next to the 64 KB tile
 static int sm_count_cached();
 static long long persistent_min_tiles();
 template <int EPI>
@@ -275,9 +301,9 @@ cudaError_t launch_gemm(const CUtensorMap* tmA, const CUtensorMap* tmB, const Ge
                         cudaStream_t stream) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0 || (p.N % 8) != 0 || (p.K % 8) != 0) return cudaErrorInvalidValue;
     if (epilogue == EPI_SWIGLU && (p.N % 32) != 0) return cudaErrorInvalidValue;
-    // large-M (prefill) shapes with the widest tile go to the persistent kernel (epilogue overlapped with the next tile)
-    if (block_n == 256 && epilogue != EPI_LOGITS && !persistent_disabled() &&
-        (long long)((p.N + 255) / 256) * ((p.M + BLOCK_M - 1) / BLOCK_M) >= persistent_min_tiles()) {
+    // large-M (prefill) shapes with the persistent kernel's tile go to it (epilogue overlapped with the next tile); tmB's box is block_n rows
+    if (block_n == PERSIST_BN && epilogue != EPI_LOGITS && !persistent_disabled() &&
+        (long long)((p.N + PERSIST_BN - 1) / PERSIST_BN) * ((p.M + BLOCK_M - 1) / BLOCK_M) >= persistent_min_tiles()) {
         switch (epilogue) {
             case EPI_STORE: return launch_persistent<EPI_STORE>(tmA, tmB, p, stream);
             case EPI_RESID: return launch_persistent<EPI_RESID>(tmA, tmB, p, stream);
@@ -294,17 +320,16 @@ cudaError_t launch_gemm(const CUtensorMap* tmA, const CUtensorMap* tmB, const Ge
 }
 
 // =============================================================================================
-// persistent tile GEMM (prefill, M > 128): one CTA per SM loops over 128 x 256 tiles in grouped raster order; TMEM holds
-// TWO accumulators so the epilogue of tile i (tcgen05.ld -> smem transpose -> coalesced bf16 stores, fused bias /
-// residual / SwiGLU) overlaps the tcgen05.mma main loop of tile i+1.
+// persistent tile GEMM (prefill, M > 128): one CTA per SM loops over 128 x 128 tiles in grouped raster order; warpgroup 1 runs the
+// wgmma main loop of tile i+1 while warpgroup 0 stores tile i.
 // =============================================================================================
 struct PersistCfg {
-    static constexpr int BN = 256;
+    static constexpr int BN = PERSIST_BN;
     static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2, B_BYTES = BN * BLOCK_K * 2, STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = 4;
-    static constexpr int EPI_ROW_FLOATS = 36, EPI_WARP_BYTES = 32 * EPI_ROW_FLOATS * 4;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 4 * EPI_WARP_BYTES + 1024 + 256;
-    static constexpr uint32_t TMEM_COLS = 512;
+    static constexpr int ACC_BYTES = BLOCK_M * BN * 4;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 + 256;
+    static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget of one CTA");
 };
 
 OA_DEVINL void raster_tile(int idx, int m_tiles, int n_tiles, int& m_blk, int& n_blk) {
@@ -316,40 +341,35 @@ OA_DEVINL void raster_tile(int idx, int m_tiles, int n_tiles, int& m_blk, int& n
 }
 
 template <int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA,
+__global__ void OA_GEMM_REGS gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                             const __grid_constant__ CUtensorMap tmB,
                                                                             const GemmParams p) {
     using Cfg = PersistCfg;
     constexpr int BN = Cfg::BN, STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* epi_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + 4 * Cfg::EPI_WARP_BYTES);
+    float* acc = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::ACC_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* acc_full = empty_bar + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+    uint64_t* acc_empty = acc_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_tiles = (p.N + BN - 1) / BN, m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
     const int total_tiles = n_tiles * m_tiles;
     const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
+        mbar_init(acc_full, CONSUMER_WARPS); mbar_init(acc_empty, 4);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_launch();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= PRODUCER_WARP) {
+        if (warp == PRODUCER_WARP && lane == 0) {
             griddep_wait();
             int s = 0; uint32_t ph = 0;
             for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -364,60 +384,32 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_persistent_kernel(const 
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BLOCK_M, BN);
-            int s = 0; uint32_t ph = 0; int it = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
-                const int as = it & 1;
-                mbar_wait(&acc_empty[as], (((uint32_t)it >> 1) & 1) ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                    const uint64_t a_desc = umma_desc_sw128(a_addr), b_desc = umma_desc_sw128(a_addr + Cfg::A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                        umma_bf16(tmem_d, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-                    umma_commit(&empty_bar[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
-                }
-                umma_commit(&acc_full[as]);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        float* stage = epi_smem + (warp - 2) * (Cfg::EPI_WARP_BYTES / 4);
-        griddep_wait();
-        int it = 0;
+    } else if (warp < CONSUMER_WARPS) {
+        int s = 0; uint32_t ph = 0, it = 0;
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
+            float d[1][BN / 2] = {};
+            wg_mma_run<BN, 1, STAGES, Cfg::STAGE_BYTES, Cfg::A_BYTES, Cfg::A_BYTES>(d, smem, full_bar, s, ph, num_kb);
+            mbar_wait(acc_empty, (it & 1) ^ 1);      // the epilogue has drained the previous tile
+            wg_acc_publish<BN, 1>(acc, d, acc_full);
+            if (warp >= 4) continue;
+            // ---------------- epilogue: warpgroup 0 ----------------
+            const int q = warp & 3;
+            griddep_wait();
             int m_blk, n_blk; raster_tile(t, m_tiles, n_tiles, m_blk, n_blk);
-            const int as = it & 1;
-            mbar_wait(&acc_full[as], ((uint32_t)it >> 1) & 1);
-            tcgen05_fence_after();
+            mbar_wait(acc_full, it & 1);
             const int row_base = m_blk * BLOCK_M + q * 32;
 #pragma unroll 1
             for (int cc = 0; cc < BN; cc += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + cc), v);
-                tmem_ld_wait();
                 const int col0 = n_blk * BN + cc;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(stage + lane * Cfg::EPI_ROW_FLOATS + j) =
-                        make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                __syncwarp();
                 if (EPI == EPI_SWIGLU) {
                     // chunk = 16 gate + 16 up columns -> 16 output features; lane = (row, 8-feature half)
                     const int h = lane & 1;
 #pragma unroll
                     for (int i2 = 0; i2 < 2; ++i2) {
                         const int r = i2 * 16 + (lane >> 1), row = row_base + r;
-                        const float* sp = stage + r * Cfg::EPI_ROW_FLOATS + h * 8;
-                        const float4 g0 = *reinterpret_cast<const float4*>(sp), g1 = *reinterpret_cast<const float4*>(sp + 4);
-                        const float4 u0 = *reinterpret_cast<const float4*>(sp + 16), u1 = *reinterpret_cast<const float4*>(sp + 20);
+                        const int ar = q * 32 + r, ac = cc + h * 8;
+                        const float4 g0 = acc_ld4(acc, BN, ar, ac), g1 = acc_ld4(acc, BN, ar, ac + 4);
+                        const float4 u0 = acc_ld4(acc, BN, ar, ac + 16), u1 = acc_ld4(acc, BN, ar, ac + 20);
                         const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
                         const float uu[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
                         float f[8];
@@ -434,8 +426,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_persistent_kernel(const 
 #pragma unroll
                     for (int i4 = 0; i4 < 4; ++i4) {
                         const int r = i4 * 8 + (lane >> 2), row = row_base + r;
-                        const float* sp = stage + r * Cfg::EPI_ROW_FLOATS + c8;
-                        const float4 a0 = *reinterpret_cast<const float4*>(sp), a1 = *reinterpret_cast<const float4*>(sp + 4);
+                        const float4 a0 = acc_ld4(acc, BN, q * 32 + r, cc + c8), a1 = acc_ld4(acc, BN, q * 32 + r, cc + c8 + 4);
                         float f[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
                         if (row < p.M && col < p.N) {
                             if (EPI == EPI_STORE) {
@@ -454,16 +445,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_persistent_kernel(const 
                         }
                     }
                 }
-                __syncwarp();
             }
-            tcgen05_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[as]);
+            if (lane == 0) mbar_arrive(acc_empty);
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) { tcgen05_fence_after(); tmem_dealloc<Cfg::TMEM_COLS>(tmem_base); }
 }
 
 static bool persistent_disabled() { static const bool off = [] { const char* e = std::getenv("OA_GEMM_PERSISTENT"); return e && e[0] == '0'; }(); return off; }
@@ -471,7 +457,7 @@ static bool persistent_disabled() { static const bool off = [] { const char* e =
 static long long persistent_min_tiles() { const char* e = std::getenv("OA_GEMM_PERSISTENT_MIN_TILES"); return e ? std::atoll(e) : 2LL * sm_count_cached(); }
 static int sm_count_cached() {
     static int n = 0;
-    if (n == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+    if (n == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
     return n;
 }
 
@@ -480,7 +466,7 @@ static cudaError_t launch_persistent(const CUtensorMap* tmA, const CUtensorMap* 
     auto kern = gemm_persistent_kernel<EPI>;
     static bool attr_done[16] = {};
     { cudaError_t e = ensure_dynamic_smem(kern, PersistCfg::SMEM_BYTES, attr_done); if (e != cudaSuccess) return e; }
-    const int tiles = ((p.N + 255) / 256) * ((p.M + BLOCK_M - 1) / BLOCK_M);
+    const int tiles = ((p.N + PersistCfg::BN - 1) / PersistCfg::BN) * ((p.M + BLOCK_M - 1) / BLOCK_M);
     const int grid = tiles < sm_count_cached() ? tiles : sm_count_cached();
     return launch_k(kern, dim3(grid), dim3(GEMM_THREADS), PersistCfg::SMEM_BYTES, stream, *tmA, *tmB, p);
 }
@@ -488,22 +474,21 @@ static cudaError_t launch_persistent(const CUtensorMap* tmA, const CUtensorMap* 
 // =============================================================================================
 // stream-K (decode, M <= 128): persistent CTAs, balanced weight streaming, fp32 partials
 // =============================================================================================
-template <int BN, int MT, int OCC = 1>     // MT = 128-row tiles of A per unit (1: M <= 128, 2: M <= 256); OCC = CTAs per SM the ring is sized for
+template <int BN, int MT>     // MT = 128-row tiles of A per unit (1: M <= 128, 2: M <= 256)
 struct SkCfg {
     static constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
     static constexpr int A_BYTES = MT * A_TILE_BYTES;
     static constexpr int B_BYTES = BN * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = (OCC == 2 ? 92 * 1024 : 200 * 1024) / STAGE_BYTES;   // 6 x 32 KB (BN=128), 4 x 48 KB (BN=256); halved for 2 CTAs/SM
-    static constexpr int EPI_ROW_FLOATS = 36;                          // 32 + 4 pad: conflict-free 16-byte smem accesses
-    static constexpr int EPI_WARP_BYTES = 32 * EPI_ROW_FLOATS * 4;     // one 32x32 fp32 chunk per epilogue warp
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 4 * EPI_WARP_BYTES + 1024 + 256;
-    static constexpr uint32_t TMEM_COLS = 2 * MT * BN;                 // two accumulator stages of MT row tiles
-    static_assert(TMEM_COLS * OCC <= 512, "TMEM holds 512 columns per SM");
+    static constexpr int ACC_BYTES = MT * BLOCK_M * BN * 4;
+    static constexpr int STAGES_FIT = (SMEM_LIMIT - ACC_BYTES - 1024 - 256) / STAGE_BYTES;
+    static constexpr int STAGES = STAGES_FIT < 6 ? STAGES_FIT : 6;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 + 256;
+    static_assert(STAGES >= 2 && SMEM_BYTES <= SMEM_LIMIT, "shared memory budget of one CTA");
 };
 
 // Epilogues finished INSIDE the stream-K GEMM by the CTA that holds a tile's first k-block (FUSE != 0): it adds the other CTAs' published
-// pieces to its TMEM accumulator in CTA order (the stand-alone consumers' order: bit-identical sums) and writes the final bf16 result.
+// pieces to its own accumulator in CTA order (the stand-alone consumers' order: bit-identical sums) and writes the final bf16 result.
 //   FUSE 1  gate/up : act = silu(gate) * up
 //   FUSE 2  o / down: x += acc            (residual stream, bf16, in place)
 //   FUSE 3  qkv     : (+ bias) -> bf16 -> RoPE -> q_out / paged K rows; V rows copied
@@ -513,40 +498,35 @@ struct SkFuse {
     SkRopeArgs rope;                    // FUSE 3
 };
 
-template <int BN, int MT, int OCC, int FUSE = 0>
-__global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const __grid_constant__ CUtensorMap tmA,
+template <int BN, int MT, int FUSE = 0>
+__global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                          const __grid_constant__ CUtensorMap tmB, const int M,
                                                                          const StreamK sk, const SkFuse fz) {
-    using Cfg = SkCfg<BN, MT, OCC>;
+    using Cfg = SkCfg<BN, MT>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* epi_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + 4 * Cfg::EPI_WARP_BYTES);
+    float* acc_s = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);    // accumulator tile [MT * 128][BN]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::ACC_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* acc_full = empty_bar + STAGES;      // [2]
-    uint64_t* acc_empty = acc_full + 2;           // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+    uint64_t* acc_full = empty_bar + STAGES;
+    uint64_t* acc_empty = acc_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long c = blockIdx.x, G = gridDim.x;
     const long long u0 = c * sk.total / G, u1 = (c + 1) * sk.total / G;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CONSUMER_WARPS); }
+        mbar_init(acc_full, CONSUMER_WARPS); mbar_init(acc_empty, 4);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     griddep_launch();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= PRODUCER_WARP) {
+        if (warp == PRODUCER_WARP && lane == 0) {
             // weights first: they depend on no predecessor, so the HBM stream starts while the previous kernel drains
             const int pre = (u1 - u0) < STAGES ? (int)(u1 - u0) : STAGES;
             for (int i = 0; i < pre; ++i) {
@@ -584,46 +564,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                 if (++s == STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BLOCK_M, BN);
-            int s = 0; uint32_t ph = 0; int seg = 0;
-            for (long long u = u0; u < u1; ++seg) {
-                const int tile = (int)(u / sk.kb);
-                const long long uend = min(u1, (long long)(tile + 1) * sk.kb);
-                const int as = seg & 1;
-                mbar_wait(&acc_empty[as], (((uint32_t)seg >> 1) & 1) ^ 1);      // epilogue has drained this accumulator
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(as * MT * BN);
-                for (long long uu = u; uu < uend; ++uu) {
-                    mbar_wait(&full_bar[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                    const uint64_t b_desc = umma_desc_sw128(a_addr + Cfg::A_BYTES);
-#pragma unroll
-                    for (int m = 0; m < MT; ++m) {
-                        const uint64_t a_desc = umma_desc_sw128(a_addr + m * Cfg::A_TILE_BYTES);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                            umma_bf16(tmem_d + (uint32_t)(m * BN), a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc, (uu > u || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
-                }
-                umma_commit(&acc_full[as]);
-                u = uend;
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        int seg = 0;
-        griddep_wait();                   // the predecessor may still be reading the partial workspace
+    } else if (warp < CONSUMER_WARPS) {
+        int s = 0; uint32_t ph = 0, seg = 0;
         for (long long u = u0; u < u1; ++seg) {
             const int tile = (int)(u / sk.kb);
             const long long uend = min(u1, (long long)(tile + 1) * sk.kb);
-            const int as = seg & 1;
-            mbar_wait(&acc_full[as], ((uint32_t)seg >> 1) & 1);
-            tcgen05_fence_after();
+            float d[MT][BN / 2] = {};
+            wg_mma_run<BN, MT, STAGES, Cfg::STAGE_BYTES, Cfg::A_TILE_BYTES, Cfg::A_BYTES>(d, smem, full_bar, s, ph, (int)(uend - u));
+            mbar_wait(acc_empty, (seg & 1) ^ 1);      // the epilogue has drained the previous segment
+            wg_acc_publish<BN, MT>(acc_s, d, acc_full);
+            if (warp >= 4) { u = uend; continue; }
+            // ---------------- epilogue: warpgroup 0 ----------------
+            const int q = warp & 3;
+            griddep_wait();                   // the predecessor may still be reading the partial workspace
+            mbar_wait(acc_full, seg & 1);
             if constexpr (FUSE == 2 || FUSE == 3) {
                 // Same publish / finish protocol as the SwiGLU epilogue below (see there for why the finishing CTA never waits on a
                 // waiting CTA); only what the finisher does with the summed 128 x 128 tile differs.
@@ -635,7 +589,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                 if ((int)c == c_first) {
                     const int n_other = c_last - c_first;
                     if (n_other > 0) {
-                        if (threadIdx.x == 64) { grid_counter_wait32(flag, (unsigned int)n_other); *flag = 0u; }
+                        if (threadIdx.x == EPI_WARP0 * 32) { grid_counter_wait32(flag, (unsigned int)n_other); *flag = 0u; }
                         asm volatile("bar.sync 1, 128;" ::: "memory");
                     }
                     const float* other = sk.ws + (size_t)(c_first + 1 + tile) * (BLOCK_M * BN) + row;
@@ -643,8 +597,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                     // acc[0..32) = this row's sums of columns [mc, mc+32) of the tile: own accumulator, then the other pieces in CTA order
                     auto acc_chunk = [&](int mc, float (&acc)[32]) {
                         uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + mc), v);
-                        tmem_ld_wait();
+                        acc_ld32(acc_s, BN, row, mc, v);
 #pragma unroll
                         for (int j = 0; j < 32; ++j) acc[j] = 0.f + __uint_as_float(v[j]);      // "0 +" as in sk_sum8
                         for (int o = 0; o < n_other; ++o) {
@@ -746,8 +699,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
 #pragma unroll 1
                     for (int mc = 0; mc < BN; mc += 32) {
                         uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + mc), v);
-                        tmem_ld_wait();
+                        acc_ld32(acc_s, BN, row, mc, v);
                         if (row < M) {
 #pragma unroll
                             for (int j = 0; j < 32; ++j) dst[(size_t)(mc + j) * BLOCK_M] = __uint_as_float(v[j]);
@@ -755,7 +707,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                     }
                     __threadfence();
                     asm volatile("bar.sync 1, 128;" ::: "memory");
-                    if (threadIdx.x == 64) atomicAdd(flag, 1u);
+                    if (threadIdx.x == EPI_WARP0 * 32) atomicAdd(flag, 1u);
                 }
             } else if constexpr (FUSE == 1) {
                 // Pieces of this tile live in CTAs c_first..c_last (same arithmetic as sk_sum8).  The CTA holding the FIRST k-block
@@ -771,7 +723,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                 if ((int)c == c_first) {
                     const int n_other = c_last - c_first;
                     if (n_other > 0) {
-                        if (threadIdx.x == 64) { grid_counter_wait32(flag, (unsigned int)n_other); *flag = 0u; }
+                        if (threadIdx.x == EPI_WARP0 * 32) { grid_counter_wait32(flag, (unsigned int)n_other); *flag = 0u; }
                         asm volatile("bar.sync 1, 128;" ::: "memory");
                     }
                     const float* other = sk.ws + (size_t)(c_first + 1 + tile) * (BLOCK_M * BN) + row;
@@ -788,8 +740,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                         const int mc = k4 * 32;
                         if (n_other > 0 && k4 + 1 < BN / 32) load_piece(t[(k4 + 1) & 1], other, mc + 32);      // next chunk's piece is in flight during this chunk's math
                         uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + mc), v);
-                        tmem_ld_wait();
+                        acc_ld32(acc_s, BN, row, mc, v);
                         float acc[32];
 #pragma unroll
                         for (int j = 0; j < 32; ++j) acc[j] = 0.f + __uint_as_float(v[j]);      // "0 +" as in sk_sum8
@@ -820,8 +771,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
 #pragma unroll 1
                     for (int mc = 0; mc < BN; mc += 32) {
                         uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + mc), v);
-                        tmem_ld_wait();
+                        acc_ld32(acc_s, BN, row, mc, v);
                         if (row < M) {
 #pragma unroll
                             for (int j = 0; j < 32; ++j) dst[(size_t)(mc + j) * BLOCK_M] = __uint_as_float(v[j]);
@@ -829,43 +779,29 @@ __global__ void __launch_bounds__(GEMM_THREADS, OCC) gemm_streamk_kernel(const _
                     }
                     __threadfence();
                     asm volatile("bar.sync 1, 128;" ::: "memory");
-                    if (threadIdx.x == 64) atomicAdd(flag, 1u);
+                    if (threadIdx.x == EPI_WARP0 * 32) atomicAdd(flag, 1u);
                 }
             } else {
-            // TMEM gives each thread one row x 32 columns; transpose through padded smem so that every global store
-            // instruction writes four full 128-byte lines (8 lanes per row) instead of 32 scattered 16-byte pieces.
-            float* stage = epi_smem + (warp - 2) * (Cfg::EPI_WARP_BYTES / 4);
+            // read the shared accumulator tile row-wise so that every global store instruction writes four full 128-byte lines
+            // (8 lanes per row)
             const int r_sub = lane >> 3, c4 = (lane & 7) * 4;
 #pragma unroll 1
             for (int mc = 0; mc < MT * BN; mc += 32) {
                 const int m = mc / BN, cc = mc - m * BN;
                 float* dst = sk.ws + ((size_t)(c + tile) * (MT * BLOCK_M) + m * BLOCK_M + q * 32) * BN;
-                uint32_t v[32];
-                tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * MT * BN + mc), v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(stage + lane * Cfg::EPI_ROW_FLOATS + j) =
-                        make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                __syncwarp();
 #pragma unroll
                 for (int it = 0; it < 8; ++it) {
                     const int r = it * 4 + r_sub;
-                    const float4 val = *reinterpret_cast<const float4*>(stage + r * Cfg::EPI_ROW_FLOATS + c4);
+                    const float4 val = acc_ld4(acc_s, BN, m * BLOCK_M + q * 32 + r, cc + c4);
                     if (m * BLOCK_M + q * 32 + r < M) *reinterpret_cast<float4*>(dst + (size_t)r * BN + cc + c4) = val;
                 }
-                __syncwarp();
             }
             }
-            tcgen05_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[as]);
+            if (lane == 0) mbar_arrive(acc_empty);
             u = uend;
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) { tcgen05_fence_after(); tmem_dealloc<Cfg::TMEM_COLS>(tmem_base); }
 }
 
 StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows) {
@@ -876,26 +812,26 @@ StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows) {
 }
 size_t streamk_ws_bytes(int N, int bn, int G, int rows) { return (size_t)(G + (N + bn - 1) / bn) * (rows > 128 ? 256 : 128) * bn * sizeof(float); }
 
-template <int BN, int MT, int OCC = 1, int FUSE = 0>
+template <int BN, int MT, int FUSE = 0>
 static cudaError_t launch_sk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, const StreamK& sk, cudaStream_t stream, SkFuse fz = SkFuse{}) {
-    auto kern = gemm_streamk_kernel<BN, MT, OCC, FUSE>;
+    auto kern = gemm_streamk_kernel<BN, MT, FUSE>;
     static bool attr_done[16] = {};
-    { cudaError_t e = ensure_dynamic_smem(kern, SkCfg<BN, MT, OCC>::SMEM_BYTES, attr_done); if (e != cudaSuccess) return e; }
-    return launch_k(kern, dim3(sk.G), dim3(GEMM_THREADS), SkCfg<BN, MT, OCC>::SMEM_BYTES, stream, *tmA, *tmB, M, sk, fz);
+    { cudaError_t e = ensure_dynamic_smem(kern, SkCfg<BN, MT>::SMEM_BYTES, attr_done); if (e != cudaSuccess) return e; }
+    return launch_k(kern, dim3(sk.G), dim3(GEMM_THREADS), SkCfg<BN, MT>::SMEM_BYTES, stream, *tmA, *tmB, M, sk, fz);
 }
 cudaError_t launch_gemm_streamk_swiglu(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int F, int K, const StreamK& sk, void* act,
                                        unsigned int* tile_flags, cudaStream_t stream) {
     if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (F % 16) != 0 || (K % 8) != 0 || !act || !tile_flags) return cudaErrorInvalidValue;
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;      // finishing CTAs wait for publishing CTAs: all must be resident
     SkFuse fz{}; fz.act = reinterpret_cast<uint16_t*>(act); fz.F = F; fz.tile_flags = tile_flags;
-    return launch_sk<128, 1, 1, 1>(tmA, tmB, M, sk, stream, fz);
+    return launch_sk<128, 1, 1>(tmA, tmB, M, sk, stream, fz);
 }
 cudaError_t launch_gemm_streamk_resid(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, void* x, int ldx,
                                       unsigned int* tile_flags, cudaStream_t stream) {
     if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (N % 32) != 0 || (K % 8) != 0 || !x || !tile_flags || (ldx % 8) != 0) return cudaErrorInvalidValue;
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;      // finishing CTAs wait for publishing CTAs: all must be resident
     SkFuse fz{}; fz.tile_flags = tile_flags; fz.x = reinterpret_cast<uint16_t*>(x); fz.ldx = ldx; fz.N = N;
-    return launch_sk<128, 1, 1, 2>(tmA, tmB, M, sk, stream, fz);
+    return launch_sk<128, 1, 2>(tmA, tmB, M, sk, stream, fz);
 }
 cudaError_t launch_gemm_streamk_rope(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, const SkRopeArgs& rope,
                                      unsigned int* tile_flags, cudaStream_t stream) {
@@ -903,14 +839,14 @@ cudaError_t launch_gemm_streamk_rope(const CUtensorMap* tmA, const CUtensorMap* 
     if ((rope.D != 64 && rope.D != 128) || N != (rope.nh + 2 * rope.nkv) * rope.D) return cudaErrorInvalidValue;      // BN must be a multiple of D; chunks of 32 never straddle a head
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;
     SkFuse fz{}; fz.tile_flags = tile_flags; fz.N = N; fz.rope = rope;
-    return launch_sk<128, 1, 1, 3>(tmA, tmB, M, sk, stream, fz);
+    return launch_sk<128, 1, 3>(tmA, tmB, M, sk, stream, fz);
 }
 cudaError_t launch_gemm_streamk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, cudaStream_t stream) {
     if (M <= 0 || M > sk.rows || (N % 8) != 0 || (K % 8) != 0) return cudaErrorInvalidValue;
     if (sk.rows == 256) return sk.bn == 128 ? launch_sk<128, 2>(tmA, tmB, M, sk, stream) : cudaErrorInvalidValue;
     if (sk.bn == 256) return launch_sk<256, 1>(tmA, tmB, M, sk, stream);
-    if (sk.bn == 128) return sk.G > sm_count_cached() ? launch_sk<128, 1, 2>(tmA, tmB, M, sk, stream) : launch_sk<128, 1, 1>(tmA, tmB, M, sk, stream);
-    if (sk.bn == 64) return launch_sk<64, 1, 1>(tmA, tmB, M, sk, stream);       // half the partial bytes again; per-projection opt-in (sk_bn_o / sk_bn_down / sk_bn_qkv)
+    if (sk.bn == 128) return launch_sk<128, 1>(tmA, tmB, M, sk, stream);      // more CTAs than SMs run in waves: the plain kernel never waits on another CTA
+    if (sk.bn == 64) return launch_sk<64, 1>(tmA, tmB, M, sk, stream);       // half the partial bytes again; per-projection opt-in (sk_bn_o / sk_bn_down / sk_bn_qkv)
     return cudaErrorInvalidValue;
 }
 

@@ -1,4 +1,4 @@
-// kernels.hpp — host-side launch API of the sm_100a kernels (csrc/*.cu).  Device pointers in,
+// kernels.hpp — host-side launch API of the sm_90a kernels (csrc/*.cu).  Device pointers in,
 // cudaError_t out; every launcher is asynchronous on the given stream.
 #pragma once
 #include <cuda.h>
@@ -14,7 +14,7 @@ namespace oa {
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
                       uint32_t box_rows, uint32_t box_cols);
 
-// ---- GEMM (gemm_tcgen05.cu): C[M,N] = A[M,K] . B[N,K]^T, bf16 in, fp32 accumulate in TMEM -------
+// ---- GEMM (gemm_tcgen05.cu): C[M,N] = A[M,K] . B[N,K]^T, bf16 in, fp32 accumulate in registers ----
 enum GemmEpilogue : int {
     EPI_STORE = 0,    // out[M,N] bf16 = acc (+ bias[N])
     EPI_RESID = 1,    // out[M,N] bf16 = acc + resid[M,N]      (out may alias resid)
@@ -159,9 +159,7 @@ struct PrefillAttnParams {
     int32_t layer, n_heads, n_kv;
     float scale_log2e;
 };
-cudaError_t launch_prefill_attention(const CUtensorMap* tm_kv, const KvLayout& kv, const PrefillAttnParams& p, cudaStream_t s);   // legacy mma.sync path
-// tcgen05 path (attention_prefill_tc.cu): tm_q = box {64 cols, 128 rows} over q[T, nh*D]
-cudaError_t launch_prefill_attention_tc(const CUtensorMap* tm_q, const CUtensorMap* tm_kv, const KvLayout& kv, const PrefillAttnParams& p, cudaStream_t s);
+cudaError_t launch_prefill_attention(const CUtensorMap* tm_kv, const KvLayout& kv, const PrefillAttnParams& p, cudaStream_t s);
 
 // bookkeeping for bench.py's gpu_launches claim
 uint64_t launches_total();

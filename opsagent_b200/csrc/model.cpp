@@ -74,7 +74,7 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     cuda_check(cudaSetDevice(opt.device), "cudaSetDevice");
     cudaDeviceProp prop;
     cuda_check(cudaGetDeviceProperties(&prop, opt.device), "cudaGetDeviceProperties");
-    if (prop.major != 10) throw std::runtime_error("opsagent_b200 requires an sm_100 (Blackwell B200) device; found sm_" +
+    if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("opsagent_b200 requires an sm_90 (Hopper H100) device; found sm_" +
                                                    std::to_string(prop.major) + std::to_string(prop.minor));
     sm_count = prop.multiProcessorCount;
     cuda_check(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking), "cudaStreamCreate");
@@ -142,7 +142,7 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
         int r = make_tmap_bf16_2d(tm, p, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, 128, 64);
         if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for an activation buffer (code " + std::to_string(r) + ")");
     };
-    amap(&tm_xn_, xn_, MR, H); amap(&tm_attn_, attn_, MR, qd); amap(&tm_act_, act_, MR, F); amap(&tm_q_, q_, MR, qd);
+    amap(&tm_xn_, xn_, MR, H); amap(&tm_attn_, attn_, MR, qd); amap(&tm_act_, act_, MR, F);
     cuda_check(cudaMemsetAsync(q_, 0, (size_t)MR * qd * 2, stream), "memset");
     // sampled rows (debug logits sample every row of a short prefill: up to 2048)
     const int MS = max_sample_;
@@ -314,16 +314,22 @@ const char* DeviceModel::kt_name(int id) {
     return n[id & 15];
 }
 void DeviceModel::sync() { cuda_check(cudaStreamSynchronize(stream), "stream sync"); }
+void DeviceModel::sampled_logits(int S, float* out) {
+    const int n_tiles = gemm_n_tiles(cfg.vocab, pick_bn(S, cfg.vocab, opt.bn_lm, false));     // the LM head's per-tile row maxima of that forward
+    std::vector<float> v((size_t)S * n_tiles);
+    cuda_check(cudaMemcpy(v.data(), amax_val_, v.size() * 4, cudaMemcpyDeviceToHost), "row maxima D2H");
+    for (int r = 0; r < S; ++r) out[r] = *std::max_element(v.begin() + (size_t)r * n_tiles, v.begin() + (size_t)(r + 1) * n_tiles);
+}
 
 // N-tile heuristic.  Decode (M <= 128) streams weights once: prefer the largest tile that still yields >= 1 CTA
 // per SM; prefill has M/128 row tiles as well, so the widest tile (least A re-reads) wins.
 int DeviceModel::pick_bn(int M, int N, int override_bn, bool swiglu) const {
     if (override_bn == 32 || override_bn == 64 || override_bn == 128 || override_bn == 256) return override_bn;
     const int m_tiles = (M + 127) / 128;
-    const int cands[4] = {256, 128, 64, 32};
-    // one or two row tiles (decode-sized batches off the stream-K path, e.g. Qwen2.5-32B TP=4 at B=256): a CTA's k-loop is latency-bound
-    // (~0.3 us per k-block), so wider tiles with fewer, longer-lived CTAs win as long as about half the SMs stream — measured per shape in
-    // profiles/r02e_gemm_shapes_m256.md (gate_up 51 -> 39 us at BN=256, down 36 -> 33 us at BN=128); many row tiles: fill every SM
+    // no 256-wide tile: its 64 x 256 fp32 fragment does not fit one consumer warpgroup's registers without spills
+    const int cands[3] = {128, 64, 32};
+    // one or two row tiles (decode-sized batches off the stream-K path, e.g. Qwen2.5-32B TP=4 at B=256): a CTA's k-loop is latency-bound,
+    // so wider tiles with fewer, longer-lived CTAs win as long as about half the SMs stream; many row tiles: fill every SM
     const long long want = m_tiles <= 2 ? sm_count / 2 : sm_count;
     for (int bn : cands) { if ((long long)((N + bn - 1) / bn) * m_tiles >= want) return bn; }
     (void)swiglu;
@@ -463,16 +469,14 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
             PrefillAttnParams a{}; a.q = q_; a.out = attn_; a.block_tables = d_bt; a.max_pages_per_seq = max_pages_per_seq;
             a.tiles = reinterpret_cast<const PrefillTile*>(d_meta_ + o_tiles); a.n_tiles = (int)in.tiles.size();
             a.layer = l; a.n_heads = nh; a.n_kv = nkv; a.scale_log2e = scale_log2e;
-            static const bool legacy = [] { const char* e = std::getenv("OA_PREFILL_ATTN"); return e && std::string(e) == "legacy"; }();
-            if (legacy) cuda_check(launch_prefill_attention(&tm_kv, kv, a, stream), "prefill attention (mma.sync)");
-            else cuda_check(launch_prefill_attention_tc(&tm_q_, &tm_kv, kv, a, stream), "prefill attention (tcgen05)");
+            cuda_check(launch_prefill_attention(&tm_kv, kv, a, stream), "prefill attention");
             MARK(4);
         }
         if (profile_attn) cudaEventRecord(ev[2 * l + 1], stream);
     };
     if (use_sk) {
         // decode-sized batch: persistent stream-K projections (fp32 partials) + fused consumers
-        auto bn_of = [&](int o) { return sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_); };   // two row tiles need BN=128 (TMEM)
+        auto bn_of = [&](int o) { return sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_); };   // two row tiles need BN=128 (registers)
         auto with_pf = [&](StreamK k) { k.l2_prefetch_units = std::max(0, opt.sk_l2_prefetch_kb * 1024 / (k.bn * 128)); return k; };
         const StreamK sk_qkv = make_streamk(sk_ws_, qkvd, H, bn_of(opt.sk_bn_qkv), sk_G_, sk_rows), sk_o = make_streamk(sk_ws_, H, qd, bn_of(opt.sk_bn_o), sk_G_, sk_rows);
         const StreamK sk_gu = make_streamk(sk_ws_, 2 * F, H, bn_of(opt.sk_bn_gu), sk_G_, sk_rows), sk_dn = make_streamk(sk_ws_, H, F, bn_of(opt.sk_bn_down), sk_G_, sk_rows);

@@ -1,5 +1,5 @@
 // model.hpp — device-resident model: weights, paged KV pool, activation buffers, TMA descriptors, and the
-// forward pass (prefill chunk or decode step) as a fixed sequence of sm_100a kernel launches on one stream.
+// forward pass (prefill chunk or decode step) as a fixed sequence of sm_90a kernel launches on one stream.
 #pragma once
 #include <memory>
 #include <string>
@@ -49,6 +49,8 @@ public:
     // synchronised.  logits_out (device fp32 [n_sample, vocab]) is optional.
     void forward(const StepInput& in, float* logits_out);
     void sync();
+    // after a completed single-GPU forward with S sampled rows: out[r] = the fp32 logit of the token row r sampled (its LM-head row maximum)
+    void sampled_logits(int S, float* out);
     int32_t* h_out_ids = nullptr;        // pinned, [max_batch or max_step_tokens]
 
     ModelConfig cfg; EngineOptions opt;
@@ -56,7 +58,7 @@ public:
     int tp = 1, tp_rank = 0, nh_l = 0, nkv_l = 0, F_l = 0, V_l = 0;
     std::unique_ptr<TpComm> comm;
     cudaStream_t stream = nullptr;
-    int num_pages = 0, max_pages_per_seq = 0, sm_count = 148;
+    int num_pages = 0, max_pages_per_seq = 0, sm_count = 132;
     int mask_words = 0, mask_slots = 0, max_mask_updates = 0;    // token-mask table geometry (words = ceil(vocab / 32))
     size_t weight_bytes = 0, kv_pool_bytes = 0;
     KvLayout kv{}; CUtensorMap tm_kv;
@@ -81,11 +83,11 @@ private:
     std::vector<void*> allocs_;
     // activations
     void *x_ = nullptr, *xn_ = nullptr, *qkv_ = nullptr, *q_ = nullptr, *attn_ = nullptr, *act_ = nullptr, *xs_ = nullptr, *xsn_ = nullptr;
-    CUtensorMap tm_xn_, tm_attn_, tm_act_, tm_xsn_, tm_q_;
+    CUtensorMap tm_xn_, tm_attn_, tm_act_, tm_xsn_;
     float* amax_val_ = nullptr; int* amax_idx_ = nullptr; int32_t* d_out_ids_ = nullptr;
     uint32_t* mask_table_ = nullptr;               // [mask_slots][mask_words] allowed-token bitsets of grammar states (filled on demand by the scheduler)
     float *part_o_ = nullptr, *part_ml_ = nullptr; int max_part_slots_ = 0;
-    float* sk_ws_ = nullptr; int sk_bn_ = 256, sk_G_ = 148;
+    float* sk_ws_ = nullptr; int sk_bn_ = 256, sk_G_ = 132;
     size_t nvls_region_ = 0;                       // bytes of one [128 rows, H] fp32 region of the NVLS multicast buffer (partials 0/1, reduced 0/1)
     unsigned int* tile_flags_ = nullptr;           // per-tile piece counters of the fused stream-K epilogues, [4 projections][SK_MAX_FLAG_TILES] (self-resetting)
     // pinned staging is double-buffered and fenced by events: the host may run ahead of the stream by a whole forward

@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(AR_THREADS) ar_nvls_resid_rmsnorm_kernel(const
 cudaError_t launch_ar_nvls_resid_rmsnorm(const void* mc_base, const void* local_base, size_t part_off, size_t red_off, size_t flag_off, int t, int rank, void* x,
                                          const void* gain, void* xn, int T, int H, float eps, cudaStream_t s, const TpComm::Signal& wait) {
     if (T <= 0) return cudaSuccess;
-    if (H % 8 != 0 || T > 148) return cudaErrorInvalidValue;            // CTAs wait for flags set by other ranks' CTAs of the same launch: keep the grid co-resident
+    if (H % 8 != 0 || T > 132) return cudaErrorInvalidValue;            // CTAs wait for flags set by other ranks' CTAs of the same launch: keep the grid co-resident
     char* mc = reinterpret_cast<char*>(const_cast<void*>(mc_base)); const char* lc = reinterpret_cast<const char*>(local_base);
     return launch_k(ar_nvls_resid_rmsnorm_kernel, dim3(T), dim3(AR_THREADS), 0, s, reinterpret_cast<const float*>(mc + part_off), reinterpret_cast<float*>(mc + red_off),
                     reinterpret_cast<const float*>(lc + red_off), reinterpret_cast<uint32_t*>(mc + flag_off), reinterpret_cast<const uint32_t*>(lc + flag_off), t, rank,
@@ -451,7 +451,7 @@ __global__ void ar_resid_bf16_kernel(const uint16_t* const* __restrict__ peer, i
 cudaError_t launch_ar_resid_bf16(void* const* d_peer, int t, void* x, int T, int H, cudaStream_t s) {
     if (T <= 0) return cudaSuccess;
     const size_t n8 = (size_t)T * H / 8;
-    const int blocks = (int)std::min<size_t>((n8 + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<size_t>((n8 + 255) / 256, 132 * 8);
     return launch_k(ar_resid_bf16_kernel, dim3(blocks), dim3(256), 0, s, reinterpret_cast<const uint16_t* const*>(d_peer), t, reinterpret_cast<uint4*>(x), n8);
 }
 
@@ -488,14 +488,14 @@ __global__ void ar2_all_gather_kernel(const uint16_t* const* __restrict__ peer, 
 cudaError_t launch_ar2_reduce_scatter(void* const* d_peer_partial, int t, int rank, void* x, void* gather_mine, int T, int H, cudaStream_t s) {
     if (T <= 0) return cudaSuccess;
     const size_t n8 = (size_t)T * H / 8;
-    const int blocks = (int)std::min<size_t>((n8 / t + 255) / 256 + 1, 148 * 8);
+    const int blocks = (int)std::min<size_t>((n8 / t + 255) / 256 + 1, 132 * 8);
     return launch_k(ar2_reduce_scatter_kernel, dim3(blocks), dim3(256), 0, s, reinterpret_cast<const uint16_t* const*>(d_peer_partial), t, rank, reinterpret_cast<uint4*>(x),
                     reinterpret_cast<uint4*>(gather_mine), n8);
 }
 cudaError_t launch_ar2_all_gather(void* const* d_peer_gather, int t, int rank, void* x, int T, int H, cudaStream_t s) {
     if (T <= 0) return cudaSuccess;
     const size_t n8 = (size_t)T * H / 8;
-    const int blocks = (int)std::min<size_t>((n8 / t + 255) / 256 + 1, 148 * 8);
+    const int blocks = (int)std::min<size_t>((n8 / t + 255) / 256 + 1, 132 * 8);
     return launch_k(ar2_all_gather_kernel, dim3(blocks), dim3(256), 0, s, reinterpret_cast<const uint16_t* const*>(d_peer_gather), t, rank, reinterpret_cast<uint4*>(x), n8);
 }
 

@@ -104,7 +104,7 @@ cudaError_t launch_sk_reduce_bf16(const StreamK& sk, void* out, int T, int N, cu
 // x[T,H] += sum over ranks of bf16 partial rows                                                          (prefill path)
 cudaError_t launch_ar_resid_bf16(void* const* d_peer, int t, void* x, int T, int H, cudaStream_t s);
 // Two-shot variant for large T (prefill chunks): the one-shot kernel above makes every rank read all t full partials — t x T x H x 2 bytes, 1.07 GB
-// per all-reduce for a Llama-3-70B TP=8 chunk of 8192 tokens, 1.2 ms on the NVLink, 160 times per chunk.  Here rank r reduces only slice r
+// per all-reduce for a Llama-3-70B TP=8 chunk of 8192 tokens, 160 times per chunk.  Here rank r reduces only slice r
 // (reduce-scatter: reads (t-1)/t of ONE partial's bytes), adds the residual and publishes the finished bf16 slice in its gather buffer; after a
 // barrier every rank copies the other t-1 slices (all-gather).  2 x (t-1)/t x T x H x 2 bytes per rank instead of (t-1) x T x H x 2; each element
 // is computed once, by its slice owner, in rank order — all ranks still hold bit-identical activations.

@@ -51,7 +51,7 @@ cudaError_t launch_init_weight(void* dst, uint64_t seed, uint64_t tensor_id, int
     uint64_t key_a = host_mix64(seed ^ (tensor_id * 0xD6E8FEB86659FD93ull));
     uint64_t key_b = tensor_id_b >= 0 ? host_mix64(seed ^ ((uint64_t)tensor_id_b * 0xD6E8FEB86659FD93ull)) : 0;
     int64_t n = rows * cols;
-    int blocks = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+    int blocks = (int)((n + 255) / 256 < 132 * 16 ? (n + 255) / 256 : 132 * 16);
     init_weight_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<uint16_t*>(dst), key_a, key_b, tensor_id_b >= 0 ? 1 : 0, rows, cols,
                                               std, mean, row_off, col_off, logical_cols);
     count_launch();

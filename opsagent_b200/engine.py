@@ -150,7 +150,9 @@ class Engine:
         return json.loads(buf.value.decode())
 
     def bench_decode(self, batch: int, ctx_len: int, steps: int, warmup: int) -> dict:
-        out = (C.c_double * 8)()
-        _check(self._L.oa_bench_decode(self._h, batch, ctx_len, steps, warmup, out, 8))
+        n = 8 + 2 * batch
+        out = (C.c_double * n)()
+        _check(self._L.oa_bench_decode(self._h, batch, ctx_len, steps, warmup, out, n))
         return {"ms_per_step": out[0], "prefill_ms": out[1], "launches_per_step": out[2], "mean_ctx": out[3],
-                "attn_ms_per_step": out[4], "algorithmic_bytes_per_step": out[5], "device_ms_per_step": out[6]}
+                "attn_ms_per_step": out[4], "algorithmic_bytes_per_step": out[5], "device_ms_per_step": out[6],
+                "last_token_ids": [int(out[8 + b]) for b in range(batch)], "last_token_logits": [out[8 + batch + b] for b in range(batch)]}

@@ -2,7 +2,7 @@
 
 ``LocalCUDAClient.Chat(model, max_tokens, prompts) -> str`` has the signature, return value and error
 behaviour of ``(*OpenAIClient).Chat`` (openai.go:69-104); instead of POSTing to a remote
-/chat/completions it calls the in-process sm_100a engine through the C ABI.  The Go binding a
+/chat/completions it calls the in-process sm_90a engine through the C ABI.  The Go binding a
 maintainer would add is shown in INTEGRATION.md (Go is not available in this image).
 
 Behaviour kept from the reference:

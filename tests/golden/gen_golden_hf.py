@@ -3,7 +3,7 @@ HF transformers LlamaForCausalLM / Qwen2ForCausalLM, fp32, CPU, greedy.
 
 The reference (myysophia/OpsAgent) ships no model arithmetic and no golden vectors for this path
 (SURVEY.md §8c), so these fixtures are the pin.  Run in the build container (needs transformers +
-torch on CPU; does NOT need /root/reference):
+torch on CPU; does NOT need the reference):
 
     python tests/golden/gen_golden_hf.py [config ...]
 

@@ -28,7 +28,9 @@ def corpus():
     """Domain text WITHOUT the four prompts the benchmark sends (a tokenizer trained on them would memorise whole sentences): the rest of
     the reference tree read at generation time (Go sources with their zh/en comments, README, configs — only the learned vocabulary is
     committed, no reference text), plus seeded synthetic manifests / kubectl / trivy / ToolPrompt JSON."""
-    ref = os.environ.get("OA_REFERENCE", "/root/reference")
+    ref = os.environ.get("OA_REFERENCE", "")
+    if not os.path.isdir(ref):
+        sys.exit("set OA_REFERENCE to a checkout of the reference (myysophia/OpsAgent @ c1109da1)")
     held_out = [open(os.path.join(HERE, "prompts", n + ".txt"), encoding="utf-8").read()
                 for n in ("executeSystemPrompt_cn", "diagnoseSystemPrompt", "analysisPrompt", "auditPrompt")]
     docs = []

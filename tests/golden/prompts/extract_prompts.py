@@ -2,13 +2,12 @@
 """Extracts the reference's system prompts VERBATIM into fixtures (contract text, SURVEY.md §8c: "the system prompts verbatim").
 
 These strings are the bytes the reference feeds the Chat seam on every request, so tests and bench.py must tokenise exactly
-them, not a paraphrase.  Run in the build container (reads /root/reference, which does not exist on the GPU box):
+them, not a paraphrase.  Run with a checkout of the reference (myysophia/OpsAgent @ c1109da1):
 
-    python tests/golden/prompts/extract_prompts.py
+    OA_REFERENCE=<path to the reference checkout> python tests/golden/prompts/extract_prompts.py
 
 Writes <name>.txt (raw UTF-8 bytes of the Go raw-string constant, no trailing newline added) and index.json
-(name -> source file:line range, byte length, sha256).  tests/test_host_logic.py checks the fixtures against index.json
-and, when /root/reference is present, against a fresh extraction.
+(name -> source file:line range, byte length, sha256).  tests/test_host_logic.py checks the fixtures against index.json.
 """
 import hashlib
 import json
@@ -17,7 +16,7 @@ import re
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get("OA_REFERENCE", "/root/reference")
+REF = os.environ.get("OA_REFERENCE", "")
 
 # constant name -> (file, how the workload uses it)
 SOURCES = {

@@ -20,7 +20,7 @@ SRC = textwrap.dedent(r'''
         int rc = oa_engine_create("{\"model\": \"no-such-model\"}", &e);
         if (rc != 400 || e != (oa_engine*)0) { printf("create rc=%d\n", rc); return 1; }
         if (!strstr(oa_last_error(), "unknown model")) { printf("error text: %s\n", oa_last_error()); return 2; }
-        if (!strstr(oa_version(), "sm_100a")) return 3;
+        if (!strstr(oa_version(), "sm_90a")) return 3;
         {   /* request struct is plain data */
             oa_msg m[2]; oa_chat_req r; oa_chat_resp out;
             memset(&r, 0, sizeof r); memset(&out, 0, sizeof out);

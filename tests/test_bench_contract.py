@@ -1,5 +1,5 @@
-"""The one-line JSON contract of bench.py, checked on the committed outputs of the last GPU run (profiles/): every key the driver
-reads is present with the right type, for both arms.  (bench.py itself needs a B200; this guards the schema on CPU.)"""
+"""The one-line JSON contract of bench.py, checked on lines recorded with this build (tests/golden/bench_*.json: the GPU arm on an H100, the CPU reference arm on 8 host cores): every key a reader of
+the line needs is present with the right type, for both arms.  (bench.py itself needs the GPU; this guards the schema on CPU.)"""
 import json
 import os
 
@@ -9,10 +9,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def load(name):
-    path = os.path.join(ROOT, "profiles", name)
-    if not os.path.exists(path):
-        pytest.skip(f"{name} not committed")
-    return json.load(open(path))
+    return json.load(open(os.path.join(ROOT, "tests", "golden", name)))
 
 
 BASE_KEYS = {"metric": str, "value": (int, float), "unit": str, "n_gpus": int, "steps": int, "warmup": int, "ms_per_step": (int, float),
@@ -33,20 +30,19 @@ def check_base(line):
     assert line["cpu_baseline"]["kind"] in ("port", "reference")
 
 
-@pytest.mark.parametrize("name", ["r01h_bench.json", "r01h_bench_dp4.json", "r02a_bench.json", "r02h_bench.json", "r02b_bench_dp4.json", "r02f_bench_dp4.json", "r02c_bench_dp8.json", "r02j_bench_dp2.json", "r02k_bench.json"])
+@pytest.mark.parametrize("name", ["bench_h100.json"])
 def test_our_arm_line(name):
     line = load(name)
-    if "dp" in name:
-        line["cpu_baseline"] = load("r01h_bench.json")["cpu_baseline"]   # the CPU leg runs at N=1 only
-    if name.startswith("r02"):
-        # round 2: the reference's own request shapes, the multi-step loop and (N >= 2) the served mix + tensor parallelism are inside the contract
+    assert "H100" in line["device"]
+    if "react" in line:
+        # the reference's own request shapes, the multi-step loop and (N >= 2) the served mix + tensor parallelism are inside the contract
         assert "verbatim" in line["e2e"]["prompts"] and set(line["e2e"]["prompt_tokens_by_kind"]) <= {"analyze", "diagnose", "execute"}
         r = line["react"]
         assert r["conversations_with_final_answer"] == r["conversations"] and 0 < r["prefix_hit_rate"] < 1 and r["react_steps_per_sec"] > 0
         if line["n_gpus"] >= 2:
             assert "configs[2]" in line["config"]["workload"] and set(line["e2e"]["prompt_tokens_by_kind"]) == {"analyze", "diagnose", "execute"}
             assert line["router"]["completed"] == line["router"]["requests"] == line["n_gpus"] * 128
-            if name >= "r02i":          # the serving block goes through the native front from r02i on
+            if "front" in line["router"]:          # the serving block goes through the native front
                 assert line["router"]["front"] == "native" and line["router"]["errors"] == [] and line["router"]["rejected_429"] == 0
             tp = line["tp"]
             assert tp["parity"]["ok"] is True and tp["parity"]["t"] == line["n_gpus"] and tp["parity"]["max_dlogit"] < 2.5e-2
@@ -68,7 +64,7 @@ def test_our_arm_line(name):
     assert r["traffic"] is None or r["traffic"] >= 0.9 * r["algorithmic_bytes_per_launch"]
 
 
-@pytest.mark.parametrize("ref,ours_name", [("r01h_bench_reference_arm.json", "r01h_bench.json"), ("r02h_bench_reference_arm.json", "r02h_bench.json")])
+@pytest.mark.parametrize("ref,ours_name", [("bench_reference_arm.json", "bench_h100.json")])
 def test_reference_arm_line(ref, ours_name):
     line = load(ref)
     check_base(line)

@@ -1,4 +1,4 @@
-"""Engine-level parity on the B200 (pytest -m gpu): the full decode path through the C ABI against the CPU
+"""Engine-level parity on the H100 (pytest -m gpu): the full decode path through the C ABI against the CPU
 oracle in bf16-faithful mode on the same seeded weights and inputs (tiny configs that share every code path
 with the 8B/32B/70B presets: GQA groups 2/4/5, head_dim 64/128, qkv bias, tied embeddings, llama3 rope scaling).
 
@@ -55,7 +55,7 @@ def test_prefill_logits_through_persistent_gemm(monkeypatch):
     """same parity with every prefill projection forced through the persistent tile GEMM (the 8B prefill path)"""
     monkeypatch.setenv("OA_GEMM_PERSISTENT_MIN_TILES", "1")
     for name in CASES:
-        spec, eng = make_engine(name, bn_qkv=256, bn_o=256, bn_gu=256, bn_down=256, max_step_tokens=512)
+        spec, eng = make_engine(name, bn_qkv=128, bn_o=128, bn_gu=128, bn_down=128, max_step_tokens=512)
         orc = O.Oracle(spec, max_pos=512, mode=1)
         rng = np.random.default_rng(11)
         toks = rng.integers(0, spec.vocab, size=300).astype(np.int32)      # T > 256: tile-GEMM path, not stream-K
@@ -82,7 +82,7 @@ def test_fused_decode_epilogues_are_bit_identical_to_separate_kernels(name):
     finishing bias + RoPE + the paged-KV write and the o / down projections finishing the residual add in their own epilogues
     (sk_fuse_epi bitmask 1 / 2 / 4; o and down are followed by a norm-only kernel with the consumer's reduction order); the gate/up projection finishing
     SwiGLU in its own epilogue (the CTA holding a tile's first k-block adds the other CTAs' pieces in CTA order).  Reduction order and consumer code are shared, so logits and generated ids must be EQUAL, not close.
-    llama-3.2-1b exercises real multi-CTA tile splits on all 148 SMs."""
+    llama-3.2-1b exercises real multi-CTA tile splits on all 132 SMs."""
     full = name == "llama-3.2-1b"
     rng = np.random.default_rng(77)
     spec = O.PRESETS[name]

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200 (pytest -m gpu): every hand-written sm_100a kernel through its C-ABI entry
+"""Kernel-level parity on the H100 (pytest -m gpu): every hand-written sm_90a kernel through its C-ABI entry
 point against (a) the CPU oracle where it has the same function and (b) a plain torch fp32 reference of the op."""
 import ctypes as C
 
@@ -160,7 +160,7 @@ def test_gemm_logits_argmax(L, M, N, K, bn):
 
 @pytest.mark.parametrize("M,N,K", [(5000, 2304, 320), (300, 1024, 512), (8192, 6144, 256)])
 def test_gemm_persistent_kernel_all_epilogues(L, M, N, K, monkeypatch):
-    """prefill path: persistent 128x256 tiles, double-buffered TMEM, transposed coalesced epilogue (forced for small shapes)"""
+    """prefill path: persistent 128x128 tiles, register + shared-memory accumulator stages, coalesced epilogue (forced for small shapes)"""
     monkeypatch.setenv("OA_GEMM_PERSISTENT_MIN_TILES", "1")
     g = torch.Generator(device="cpu").manual_seed(M + N)
     A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16).to(dev())
@@ -168,19 +168,19 @@ def test_gemm_persistent_kernel_all_epilogues(L, M, N, K, monkeypatch):
     bias = torch.randn(N, generator=g).to(torch.bfloat16).to(dev())
     ref = A.float() @ B.float().T
     out = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=dev())
-    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_STORE, 256, ptr(out), ptr(bias), None, None, None, None) == 0
+    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_STORE, 128, ptr(out), ptr(bias), None, None, None, None) == 0
     torch.cuda.synchronize()
     r = ref + bias.float()
     assert torch.isfinite(out.float()).all()
     assert ((out.float() - r).abs() <= r.abs() * 2.0 ** -8 * 1.01 + 2e-3).all()
     x = torch.randn(M, N, generator=g).to(torch.bfloat16).to(dev())
     refx = (ref + x.float()).to(torch.bfloat16)
-    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_RESID, 256, ptr(x), None, ptr(x), None, None, None) == 0
+    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_RESID, 128, ptr(x), None, ptr(x), None, None, None) == 0
     torch.cuda.synchronize()
     assert ((x.float() - refx.float()).abs() <= refx.float().abs() * 2.0 ** -7 + 1e-3).all()
     F = N // 2
     out2 = torch.full((M, F), float("nan"), dtype=torch.bfloat16, device=dev())
-    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_SWIGLU, 256, ptr(out2), None, None, None, None, None) == 0
+    assert L.oa_k_gemm(ptr(A), ptr(B), M, N, K, EPI_SWIGLU, 128, ptr(out2), None, None, None, None, None) == 0
     torch.cuda.synchronize()
     acc = ref.view(M, N // 32, 2, 16)
     rs = (torch.nn.functional.silu(acc[:, :, 0]) * acc[:, :, 1]).reshape(M, F)
@@ -194,7 +194,7 @@ def test_gemm_persistent_kernel_all_epilogues(L, M, N, K, monkeypatch):
                                       (256, 4096, 4096, 148), (200, 1792, 5120, 148), (129, 320, 320, 7)])
 def test_gemm_streamk_partials_sum_to_the_product(L, M, N, K, G, bn):
     if M > 128 and bn != 128:
-        pytest.skip("two 128-row tiles need BN=128 (TMEM columns)")
+        pytest.skip("two 128-row tiles need BN=128 (accumulator registers)")
     g = torch.Generator(device="cpu").manual_seed(N + K + bn + G)
     A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16).to(dev())
     B = (torch.randn(N, K, generator=g) * 0.5).to(torch.bfloat16).to(dev())

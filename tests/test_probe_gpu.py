@@ -1,7 +1,7 @@
 """Engine configurations checked in their own process (tests/probe_worker.py): GQA group 8 — what one rank of Llama-3-70B TP=8 runs —
 and group 1, an engine whose text goes through a trained byte-level BPE tokenizer, and the scheduler's mixed steps (decoding sequences
 ride along in prefill steps: both attention kernels in one forward, staggered arrivals as the reference's one-goroutine-per-request
-callers produce them — pkg/handlers/execute.go:205).  Seen green on a B200 in round 1 (g8, mha, bpe) and round 2 (mixed): hard tests."""
+callers produce them — pkg/handlers/execute.go:205)."""
 import os
 import subprocess
 import sys

@@ -1,6 +1,6 @@
 """Host-side race / memory-error detection (SURVEY.md 5.2): the native HTTP front under TSAN and ASAN+UBSAN with a stub engine, and the parsers of
 untrusted bytes (BPE, tokenizer.json, config JSON, safetensors headers, the ToolPrompt automaton + token masks) under ASAN+UBSAN.  The device side is
-covered by compute-sanitizer on the GPU box: tools/sanitize_gpu.sh, results in profiles/r02j_sanitizers.md."""
+covered by compute-sanitizer on a GPU machine: tools/sanitize_gpu.sh."""
 import pytest
 
 # ---- race / memory-error detection on the host side (SURVEY.md 5.2) -----------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """Kernel-level sweep of the tile GEMM's N-tile choice for decode-sized batches that fall off the stream-K path (128 < M <= 256):
-Qwen2.5-32B TP=4 at B=256 runs its projections on gemm_tcgen05_kernel (one CTA per 128 x BN tile), where 112-216 CTAs on 148 SMs
+Qwen2.5-32B TP=4 at B=256 runs its projections on gemm_wgmma_kernel (one CTA per 128 x BN tile), where a few hundred CTAs on 132 SMs
 lose up to half a wave.  For each per-rank shape and BN in {32, 64, 128, 256}: CUDA-event time over rotating weight copies (so that
 weights come from HBM, as in a real step), against the weight-streaming floor.   python tools/gemm_shape_sweep.py [M]"""
 import ctypes as C

@@ -1,5 +1,5 @@
 #!/bin/bash
-# memcheck with real multi-CTA tile splits: llama-3.2-1b puts stream-K pieces of one tile on several of the 148 SMs, so the per-tile flags and the
+# memcheck with real multi-CTA tile splits: llama-3.2-1b puts stream-K pieces of one tile on several of the 132 SMs, so the per-tile flags and the
 # CTA-ordered sums of the default (fused SwiGLU) path run under the sanitizer's perturbed timing; variants must stay bit-identical.
 export PYTORCH_NO_CUDA_MEMORY_CACHING=1 OA_SKIP_SLOW_PARITY=1
 mkdir -p gpurun_out

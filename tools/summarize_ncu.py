@@ -1,6 +1,6 @@
-"""Summarise ncu outputs into profiles/ (tracked):
-   python tools/summarize_ncu.py launches gpurun_out/launches_X.csv profiles/rNN_launches.md [n_steps]
-   python tools/summarize_ncu.py report   gpurun_out/prof_X.ncu-rep profiles/rNN_kernels.md
+"""Summarise ncu outputs as markdown tables:
+   python tools/summarize_ncu.py launches <ncu --csv launch list> <out.md> [n_steps]
+   python tools/summarize_ncu.py report   <report.ncu-rep> <out.md>
 """
 import collections
 import csv
