@@ -33,6 +33,69 @@ OA_DEVINL uint32_t pack_bf16x2(float a, float b) {
     return r;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Epilogue arithmetic on 8 bf16 lanes (one 16-byte vector).  Every GEMM epilogue and every consumer kernel finishes its values
+// with these, so the fused and the stand-alone paths perform the same fp32 operations in the same order (bit-identical results).
+// ---------------------------------------------------------------------------------------------
+OA_DEVINL void unpack_bf16x8(uint4 u, float* f) {
+    f[0] = bf16lo(u.x); f[1] = bf16hi(u.x); f[2] = bf16lo(u.y); f[3] = bf16hi(u.y);
+    f[4] = bf16lo(u.z); f[5] = bf16hi(u.z); f[6] = bf16lo(u.w); f[7] = bf16hi(u.w);
+}
+OA_DEVINL uint4 pack_bf16x8(const float* f) {
+    uint4 o;
+    o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]); o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
+    return o;
+}
+// f[i] += bf16 lane i of u (bias or residual)
+OA_DEVINL void add_bf16x8(float* f, uint4 u) {
+    f[0] += bf16lo(u.x); f[1] += bf16hi(u.x); f[2] += bf16lo(u.y); f[3] += bf16hi(u.y);
+    f[4] += bf16lo(u.z); f[5] += bf16hi(u.z); f[6] += bf16lo(u.w); f[7] += bf16hi(u.w);
+}
+// f[i] = bf16(f[i]) as fp32: a projection output that is a bf16 tensor
+OA_DEVINL void round_bf16x8(float* f) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = bf16_bits_to_f32(f32_to_bf16_bits(f[k]));
+}
+// silu(g) * u, packed
+OA_DEVINL uint4 swiglu_bf16x8(const float* g, const float* u) {
+    float f[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = __fdividef(g[k], 1.0f + __expf(-g[k])) * u[k];
+    return pack_bf16x8(f);
+}
+// RoPE (rotate-half pairing) of 8 (lo, hi) pairs with cos / sin rows cs, sn (16-byte aligned): lo·c − hi·s and hi·c + lo·s, packed
+OA_DEVINL void rope_bf16x8(const float* lo, const float* hi, const float* cs, const float* sn, uint4& out_lo, uint4& out_hi) {
+    const float4 c0 = *reinterpret_cast<const float4*>(cs), c1 = *reinterpret_cast<const float4*>(cs + 4);
+    const float4 s0 = *reinterpret_cast<const float4*>(sn), s1 = *reinterpret_cast<const float4*>(sn + 4);
+    const float cv[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+    const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+    float ra[8], rb[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { ra[k] = lo[k] * cv[k] - hi[k] * sv[k]; rb[k] = hi[k] * cv[k] + lo[k] * sv[k]; }
+    out_lo = pack_bf16x8(ra);
+    out_hi = pack_bf16x8(rb);
+}
+// RMSNorm: ss + the squares of the 8 lanes of v, in lane order; and pack(v * r * g)
+OA_DEVINL float sumsq_bf16x8(uint4 v, float ss) {
+    float f[8];
+    unpack_bf16x8(v, f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) ss += f[k] * f[k];
+    return ss;
+}
+OA_DEVINL uint4 rms_scale_bf16x8(uint4 v, float r, uint4 g) {
+    float a[8], b[8];
+    unpack_bf16x8(v, a);
+    unpack_bf16x8(g, b);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) a[k] = a[k] * r * b[k];
+    return pack_bf16x8(a);
+}
+// first element of row (page, kv head, offset in page) of a K or V plane starting at row plane_row0 of the paged cache (rows of D)
+OA_DEVINL uint16_t* kv_row(uint16_t* kv_base, int64_t plane_row0, int page, int nkv, int head, int page_size, int off, int D) {
+    return kv_base + (size_t)(plane_row0 + ((int64_t)page * nkv + head) * page_size + off) * D;
+}
+
 OA_DEVINL uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // ---------------------------------------------------------------------------------------------
 // Programmatic dependent launch: every kernel of the forward chain is launched with
@@ -297,6 +360,28 @@ OA_DEVINL float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// Arg-max of row `row` of per-tile (value, column) partials [rows, n_tiles] over one block of <= 256 threads: the larger value wins, the
+// lower column on ties.  The result is in thread 0's (bv, bi); bi = 0x7fffffff when the row has no candidate.
+OA_DEVINL void block_argmax_row(const float* __restrict__ val, const int* __restrict__ idx, int row, int n_tiles, float& bv, int& bi) {
+    bv = -INFINITY; bi = 0x7fffffff;
+    for (int t = threadIdx.x; t < n_tiles; t += blockDim.x) {
+        const float v = val[(size_t)row * n_tiles + t]; const int i = idx[(size_t)row * n_tiles + t];
+        if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    __shared__ float sv[8]; __shared__ int si[8];
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = bv; si[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+            if (sv[w] > bv || (sv[w] == bv && si[w] < bi)) { bv = sv[w]; bi = si[w]; }
+    }
 }
 
 // 16-byte global accesses

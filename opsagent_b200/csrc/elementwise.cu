@@ -47,11 +47,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ 
         int i = threadIdx.x + k * 256;
         if (i < H8) {
             v[k] = xr[i];
-            float a;
-            a = bf16lo(v[k].x); ss += a * a; a = bf16hi(v[k].x); ss += a * a;
-            a = bf16lo(v[k].y); ss += a * a; a = bf16hi(v[k].y); ss += a * a;
-            a = bf16lo(v[k].z); ss += a * a; a = bf16hi(v[k].z); ss += a * a;
-            a = bf16lo(v[k].w); ss += a * a; a = bf16hi(v[k].w); ss += a * a;
+            ss = sumsq_bf16x8(v[k], ss);
         }
     }
     ss = warp_sum(ss);
@@ -66,14 +62,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ 
 #pragma unroll
     for (int k = 0; k < VPT; ++k) {
         int i = threadIdx.x + k * 256;
-        if (i < H8) {
-            uint4 gg = g[i], o;
-            o.x = pack_bf16x2(bf16lo(v[k].x) * r * bf16lo(gg.x), bf16hi(v[k].x) * r * bf16hi(gg.x));
-            o.y = pack_bf16x2(bf16lo(v[k].y) * r * bf16lo(gg.y), bf16hi(v[k].y) * r * bf16hi(gg.y));
-            o.z = pack_bf16x2(bf16lo(v[k].z) * r * bf16lo(gg.z), bf16hi(v[k].z) * r * bf16hi(gg.z));
-            o.w = pack_bf16x2(bf16lo(v[k].w) * r * bf16lo(gg.w), bf16hi(v[k].w) * r * bf16hi(gg.w));
-            yr[i] = o;
-        }
+        if (i < H8) yr[i] = rms_scale_bf16x8(v[k], r, g[i]);
     }
 }
 cudaError_t launch_rmsnorm(const void* x, const void* gain, void* y, int T, int H, float eps, cudaStream_t s) {
@@ -87,61 +76,41 @@ cudaError_t launch_rmsnorm(const void* x, const void* gain, void* y, int T, int 
 }
 
 // One CTA per token.  Thread i handles the rotate-half pair group (8 consecutive i in [0,D/2) and the
-// matching 8 in [D/2,D)) of one head: two 16-byte loads, two 16-byte stores.
-__global__ void rope_kv_write_kernel(const uint16_t* __restrict__ qkv, const int32_t* __restrict__ positions,
-                                     const int32_t* __restrict__ slots, const float* __restrict__ rope_cos,
-                                     const float* __restrict__ rope_sin, uint16_t* __restrict__ q_out, uint16_t* __restrict__ kv_base,
-                                     int64_t k_plane_row0, int64_t v_plane_row0, int page_size, int nh, int nkv, int D) {
+// matching 8 in [D/2,D)) of one head: two 16-byte loads, two 16-byte stores.  a.bias is unused: qkv already holds the biased projection.
+__global__ void rope_kv_write_kernel(const uint16_t* __restrict__ qkv, const SkRopeArgs a) {
     griddep_launch(); griddep_wait();
     const int t = blockIdx.x;
-    const int half = D >> 1, vec_per_head = half >> 3;        // 8 pairs per thread
-    const int qkv_w = (nh + 2 * nkv) * D;
-    const uint16_t* row = qkv + (size_t)t * qkv_w;
-    const int pos = positions[t];
-    const int slot = slots[t];
-    const int page = slot / page_size, off = slot - page * page_size;
-    const float* cr = rope_cos + (size_t)pos * half;
-    const float* sr = rope_sin + (size_t)pos * half;
-    const int n_rot = (nh + nkv) * vec_per_head;
+    const int D = a.D, half = D >> 1, vec_per_head = half >> 3;        // 8 pairs per thread
+    const uint16_t* row = qkv + (size_t)t * (a.nh + 2 * a.nkv) * D;
+    const int pos = a.positions[t];
+    const int slot = a.slots[t];
+    const int page = slot / a.page_size, off = slot - page * a.page_size;
+    const float* cr = a.rope_cos + (size_t)pos * half;
+    const float* sr = a.rope_sin + (size_t)pos * half;
+    const int n_rot = (a.nh + a.nkv) * vec_per_head;
     for (int w = threadIdx.x; w < n_rot; w += blockDim.x) {
         const int head = w / vec_per_head, i0 = (w - head * vec_per_head) * 8;
         const uint16_t* src = row + (size_t)head * D;
-        uint4 a = *reinterpret_cast<const uint4*>(src + i0);
-        uint4 b = *reinterpret_cast<const uint4*>(src + i0 + half);
-        float4 c0 = *reinterpret_cast<const float4*>(cr + i0), c1 = *reinterpret_cast<const float4*>(cr + i0 + 4);
-        float4 s0 = *reinterpret_cast<const float4*>(sr + i0), s1 = *reinterpret_cast<const float4*>(sr + i0 + 4);
-        float av[8] = {bf16lo(a.x), bf16hi(a.x), bf16lo(a.y), bf16hi(a.y), bf16lo(a.z), bf16hi(a.z), bf16lo(a.w), bf16hi(a.w)};
-        float bv[8] = {bf16lo(b.x), bf16hi(b.x), bf16lo(b.y), bf16hi(b.y), bf16lo(b.z), bf16hi(b.z), bf16lo(b.w), bf16hi(b.w)};
-        float cv[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-        float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-        float ra[8], rb[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) { ra[k] = av[k] * cv[k] - bv[k] * sv[k]; rb[k] = bv[k] * cv[k] + av[k] * sv[k]; }
-        uint4 oa, ob;
-        oa.x = pack_bf16x2(ra[0], ra[1]); oa.y = pack_bf16x2(ra[2], ra[3]); oa.z = pack_bf16x2(ra[4], ra[5]); oa.w = pack_bf16x2(ra[6], ra[7]);
-        ob.x = pack_bf16x2(rb[0], rb[1]); ob.y = pack_bf16x2(rb[2], rb[3]); ob.z = pack_bf16x2(rb[4], rb[5]); ob.w = pack_bf16x2(rb[6], rb[7]);
-        uint16_t* dst;
-        if (head < nh) dst = q_out + (size_t)t * nh * D + (size_t)head * D;
-        else dst = kv_base + (size_t)(k_plane_row0 + ((int64_t)page * nkv + (head - nh)) * page_size + off) * D;
-        *reinterpret_cast<uint4*>(dst + i0) = oa;
-        *reinterpret_cast<uint4*>(dst + i0 + half) = ob;
+        float av[8], bv[8];
+        unpack_bf16x8(*reinterpret_cast<const uint4*>(src + i0), av);
+        unpack_bf16x8(*reinterpret_cast<const uint4*>(src + i0 + half), bv);
+        uint16_t* dst = rope_dst_row(a, t, head, page, off);
+        rope_bf16x8(av, bv, cr + i0, sr + i0, *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
     }
     // V: straight copy into the V plane
-    const int n_v = nkv * (D >> 3);
+    const int n_v = a.nkv * (D >> 3);
     for (int w = threadIdx.x; w < n_v; w += blockDim.x) {
         const int head = w / (D >> 3), i0 = (w - head * (D >> 3)) * 8;
-        uint4 vv = *reinterpret_cast<const uint4*>(row + (size_t)(nh + nkv + head) * D + i0);
-        uint16_t* dst = kv_base + (size_t)(v_plane_row0 + ((int64_t)page * nkv + head) * page_size + off) * D;
-        *reinterpret_cast<uint4*>(dst + i0) = vv;
+        *reinterpret_cast<uint4*>(rope_dst_row(a, t, a.nh + a.nkv + head, page, off) + i0) =
+            *reinterpret_cast<const uint4*>(row + (size_t)(a.nh + a.nkv + head) * D + i0);
     }
 }
 cudaError_t launch_rope_kv_write(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos,
                                  const float* rope_sin, void* q_out, const KvLayout& kv, int layer, int T, int nh, cudaStream_t s) {
     if (T <= 0) return cudaSuccess;
     if (kv.head_dim % 16 != 0) return cudaErrorInvalidValue;
-    const int64_t k0 = (int64_t)layer * kv.layer_stride_rows, v0 = k0 + kv.kv_stride_rows;
-    return launch_k(rope_kv_write_kernel, dim3(T), dim3(256), 0, s, reinterpret_cast<const uint16_t*>(qkv), positions, slots, rope_cos, rope_sin,
-                    reinterpret_cast<uint16_t*>(q_out), reinterpret_cast<uint16_t*>(kv.base), k0, v0, kv.page_size, nh, kv.n_kv, kv.head_dim);
+    return launch_k(rope_kv_write_kernel, dim3(T), dim3(256), 0, s, reinterpret_cast<const uint16_t*>(qkv),
+                    make_sk_rope_args(nullptr, positions, slots, rope_cos, rope_sin, q_out, kv, layer, nh));
 }
 
 

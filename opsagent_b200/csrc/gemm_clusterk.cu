@@ -14,16 +14,17 @@
 // (parity against the oracle holds with the same tolerance; the bit-identity test covers the stream-K variants among themselves).
 #include <algorithm>
 
-#include "common.cuh"
-#include "kernels.hpp"
+#include "gemm_pipe.cuh"
+#include "sk_consumers.cuh"
 
 namespace oa {
 
-static constexpr int CK_BM = 128, CK_BN = 128, CK_BK = 64, CK_STAGES = 4;
-static constexpr int CK_CONSUMER_WARPS = 8, CK_THREADS = 32 * (CK_CONSUMER_WARPS + 1);
-static constexpr int CK_A_BYTES = CK_BM * CK_BK * 2, CK_B_BYTES = CK_BN * CK_BK * 2, CK_STAGE_BYTES = CK_A_BYTES + CK_B_BYTES;
+static constexpr int CK_BN = 128;
 static constexpr int CK_ROW_F = 36;                              // 32 + 4 pad floats: conflict-free 16-byte accesses
 static constexpr int CK_BUF_F = 32 * CK_ROW_F;                   // one 32 x 32 partial chunk
+template <int S> constexpr int CK_SLOTS = (8 + S - 1) / S;      // pair units a CTA may own
+// the accumulator region is the receive buffer [SLOTS][2 members][S partials][32][36]
+template <int S> using CkCfg = RingCfg<CK_BN, 1, 4, CK_SLOTS<S> * 2 * S * CK_BUF_F * 4>;
 
 struct CkEpi {
     int kind;                           // 2: x[M, ldx] += acc (residual stream, bf16, in place)   3: bias + RoPE + paged-KV write
@@ -45,69 +46,33 @@ template <int D> OA_DEVINL void ck_pair_of(int c, int& pidx, int& member) { if (
 template <int D> OA_DEVINL int ck_chunk_of(int pidx, int member) { return D == 128 ? pidx + 2 * member : 2 * pidx + member; }
 
 template <int S, int D>
-__global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                                                                      const int M, const int K, const CkEpi ep) {
-    constexpr int SLOTS = (8 + S - 1) / S;                                   // pair units a CTA may own
-    extern __shared__ __align__(1024) uint8_t smem[];
-    float* recv = reinterpret_cast<float*>(smem + CK_STAGES * CK_STAGE_BYTES);          // [SLOTS][2 members][S partials][32][36]
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(recv + SLOTS * 2 * S * CK_BUF_F);
-    uint64_t* empty_bar = full_bar + CK_STAGES;
+__global__ void OA_GEMM_REGS gemm_clusterk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                                  const int M, const int K, const CkEpi ep) {
+    using Cfg = CkCfg<S>;
+    constexpr int SLOTS = CK_SLOTS<S>;
+    extern __shared__ uint8_t smem_raw[];
+    const Ring ring = ring_setup<Cfg>(smem_raw, &tmA, &tmB);
+    float* recv = ring.acc;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t rank = ck_cluster_rank();
     const int tile = (int)blockIdx.x / S;
-    const int kb_total = (K + CK_BK - 1) / CK_BK;
+    const int kb_total = (K + BLOCK_K - 1) / BLOCK_K;
     const int kb0 = (int)((long long)rank * kb_total / S), kb1 = (int)((long long)(rank + 1) * kb_total / S), n_kb = kb1 - kb0;   // host: kb_total >= S
 
-    if (warp == CK_CONSUMER_WARPS && lane == 0) {
-        tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-        for (int s = 0; s < CK_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CK_CONSUMER_WARPS); }
-        fence_barrier_init();
-    }
-    __syncthreads();
-    griddep_launch();
-
-    float d[CK_BN / 2] = {};
-    if (warp == CK_CONSUMER_WARPS) {
+    float d[1][CK_BN / 2] = {};
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {
-            const int pre = n_kb < CK_STAGES ? n_kb : CK_STAGES;
-            for (int i = 0; i < pre; ++i) {          // weights first: the HBM stream starts while the predecessor drains
-                mbar_expect_tx(&full_bar[i], CK_STAGE_BYTES);
-                tma_load_2d(smem + i * CK_STAGE_BYTES + CK_A_BYTES, &tmB, &full_bar[i], (kb0 + i) * CK_BK, tile * CK_BN, kEvictFirst);
-            }
-            griddep_wait();
-            for (int i = 0; i < pre; ++i) tma_load_2d(smem + i * CK_STAGE_BYTES, &tmA, &full_bar[i], (kb0 + i) * CK_BK, 0, kEvictLast);
-            int s = pre == CK_STAGES ? 0 : pre; uint32_t ph = pre == CK_STAGES ? 1 : 0;
-            for (int i = pre; i < n_kb; ++i) {
-                mbar_wait(&empty_bar[s], ph ^ 1);
-                uint8_t* dst = smem + s * CK_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], CK_STAGE_BYTES);
-                tma_load_2d(dst, &tmA, &full_bar[s], (kb0 + i) * CK_BK, 0, kEvictLast);
-                tma_load_2d(dst + CK_A_BYTES, &tmB, &full_bar[s], (kb0 + i) * CK_BK, tile * CK_BN, kEvictFirst);
-                if (++s == CK_STAGES) { s = 0; ph ^= 1; }
-            }
+            auto unit = [&](int i, int& kx, int& a_row, int& b_row) { kx = (kb0 + i) * BLOCK_K; a_row = 0; b_row = tile * CK_BN; };
+            ring_produce<Cfg, true>(ring, &tmA, &tmB, n_kb, unit, kEvictLast, kEvictFirst);
         }
-    } else if (warp < CK_CONSUMER_WARPS) {
-        const int g = warp >> 2;
-        int s = 0; uint32_t ph = 0, prev = ~0u;
-        for (int i = 0; i < n_kb; ++i) {
-            mbar_wait(&full_bar[s], ph);
-            const uint32_t st = smem_u32(smem + s * CK_STAGE_BYTES);
-            const uint64_t da = gmma_desc_sw128(st + (uint32_t)(g * 64 * 128)), db = gmma_desc_sw128(st + CK_A_BYTES);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < CK_BK / 16; ++k) wgmma_bf16<CK_BN>(d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (i | k) != 0 ? 1u : 0u);
-            wgmma_commit();
-            wgmma_wait<1>();                                      // one group in flight; the previous slot is free
-            if (prev != ~0u && lane == 0) mbar_arrive(&empty_bar[prev]);
-            prev = (uint32_t)s;
-            if (++s == CK_STAGES) { s = 0; ph ^= 1; }
-        }
-        wgmma_wait<0>();
+    } else if (warp < CONSUMER_WARPS) {
+        int s = 0; uint32_t ph = 0;
+        wg_mma_run<Cfg>(d, ring, s, ph, n_kb);
     }
     // every CTA of the cluster is running (co-scheduled) and past its setup before anybody writes into a peer's shared memory
     ck_cluster_sync();
-    if (warp < CK_CONSUMER_WARPS) {
+    if (warp < CONSUMER_WARPS) {
         // fragment (row, col pair) -> the pair unit that owns it, in the owner CTA's receive buffer
         griddep_wait();
         const int g = warp >> 2, w = warp & 3;
@@ -120,7 +85,7 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
                 const int row = g * 64 + 16 * w + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
                 const int pu = (row >> 5) * 2 + pidx, owner = pu % S, slot = pu / S;
                 const uint32_t local = recv_base + (uint32_t)((((slot * 2 + member) * S + (int)rank) * CK_BUF_F + (row & 31) * CK_ROW_F + (col & 31)) * 4);
-                ck_st_cluster_f2(ck_mapa(local, (uint32_t)owner), d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+                ck_st_cluster_f2(ck_mapa(local, (uint32_t)owner), d[0][4 * j + 2 * h], d[0][4 * j + 2 * h + 1]);
             }
         }
     }
@@ -155,72 +120,34 @@ __global__ void __launch_bounds__(CK_THREADS, 1) gemm_clusterk_kernel(const __gr
                     const int col = m ? col_hi : col_lo;
                     if (col >= ep.N) continue;
                     uint4* xp = reinterpret_cast<uint4*>(ep.x + (size_t)row * ep.ldx + col);
-                    const uint4 xo = *xp; uint4 xn;
-                    xn.x = pack_bf16x2(bf16lo(xo.x) + acc[m][0], bf16hi(xo.x) + acc[m][1]); xn.y = pack_bf16x2(bf16lo(xo.y) + acc[m][2], bf16hi(xo.y) + acc[m][3]);
-                    xn.z = pack_bf16x2(bf16lo(xo.z) + acc[m][4], bf16hi(xo.z) + acc[m][5]); xn.w = pack_bf16x2(bf16lo(xo.w) + acc[m][6], bf16hi(xo.w) + acc[m][7]);
-                    *xp = xn;
+                    add_bf16x8(acc[m], *xp);
+                    *xp = pack_bf16x8(acc[m]);
                 }
             } else {
                 if (col_lo >= ep.N) continue;
                 const SkRopeArgs& a = ep.rope;
                 const int half = D >> 1, head = col_lo / D, i0 = col_lo - head * D;          // i0 in [0, D/2): the low half of a rotation pair
                 const int slot_tok = a.slots[row], page = slot_tok / a.page_size, off = slot_tok - page * a.page_size;
-#pragma unroll
-                for (int m = 0; m < 2; ++m) {                     // + bias, round: the projection output is a bf16 tensor
-                    const int col = m ? col_hi : col_lo;
-                    if (a.bias) {
-                        const uint4 bb = *reinterpret_cast<const uint4*>(a.bias + col);
-                        acc[m][0] += bf16lo(bb.x); acc[m][1] += bf16hi(bb.x); acc[m][2] += bf16lo(bb.y); acc[m][3] += bf16hi(bb.y);
-                        acc[m][4] += bf16lo(bb.z); acc[m][5] += bf16hi(bb.z); acc[m][6] += bf16lo(bb.w); acc[m][7] += bf16hi(bb.w);
-                    }
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) acc[m][i] = bf16_bits_to_f32(f32_to_bf16_bits(acc[m][i]));
-                }
-                auto pack8 = [](const float (&v)[8]) { uint4 o; o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]); o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]); return o; };
+                qkv_finish8(a.bias, col_lo, acc[0]);
+                qkv_finish8(a.bias, col_hi, acc[1]);
+                uint16_t* dst = rope_dst_row(a, row, head, page, off);
                 if (head >= a.nh + a.nkv) {                       // V: straight copy of both halves into the V plane
-                    uint16_t* dst = a.kv_base + (size_t)(a.v_plane_row0 + ((int64_t)page * a.nkv + (head - a.nh - a.nkv)) * a.page_size + off) * D;
-                    *reinterpret_cast<uint4*>(dst + i0) = pack8(acc[0]);
-                    *reinterpret_cast<uint4*>(dst + i0 + half) = pack8(acc[1]);
+                    *reinterpret_cast<uint4*>(dst + i0) = pack_bf16x8(acc[0]);
+                    *reinterpret_cast<uint4*>(dst + i0 + half) = pack_bf16x8(acc[1]);
                 } else {
                     const int pos = a.positions[row];
-                    const float* cr = a.rope_cos + (size_t)pos * half + i0;
-                    const float* sr = a.rope_sin + (size_t)pos * half + i0;
-                    const float4 c0 = *reinterpret_cast<const float4*>(cr), c1 = *reinterpret_cast<const float4*>(cr + 4);
-                    const float4 s0 = *reinterpret_cast<const float4*>(sr), s1 = *reinterpret_cast<const float4*>(sr + 4);
-                    const float cv[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w}, sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                    float ra[8], rb[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) { ra[i] = acc[0][i] * cv[i] - acc[1][i] * sv[i]; rb[i] = acc[1][i] * cv[i] + acc[0][i] * sv[i]; }
-                    uint16_t* dst;
-                    if (head < a.nh) dst = a.q_out + (size_t)row * a.nh * D + (size_t)head * D;
-                    else dst = a.kv_base + (size_t)(a.k_plane_row0 + ((int64_t)page * a.nkv + (head - a.nh)) * a.page_size + off) * D;
-                    *reinterpret_cast<uint4*>(dst + i0) = pack8(ra);
-                    *reinterpret_cast<uint4*>(dst + i0 + half) = pack8(rb);
+                    rope_bf16x8(acc[0], acc[1], a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0,
+                                *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
                 }
             }
         }
     }
 }
 
-template <int S>
-static constexpr int ck_smem_bytes() { return CK_STAGES * CK_STAGE_BYTES + ((8 + S - 1) / S) * 2 * S * CK_BUF_F * 4 + 256; }
-
 template <int S, int D>
 static cudaError_t launch_ck(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const CkEpi& ep, cudaStream_t stream) {
-    auto kern = gemm_clusterk_kernel<S, D>;
-    constexpr int SMEM = ck_smem_bytes<S>();
-    static_assert(SMEM <= 232448, "shared memory budget of one CTA");
-    static bool attr_done[16] = {};
-    { cudaError_t e = ensure_dynamic_smem(kern, SMEM, attr_done); if (e != cudaSuccess) return e; }
     const int n_tiles = (N + CK_BN - 1) / CK_BN;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_tiles * S); cfg.blockDim = dim3(CK_THREADS); cfg.dynamicSmemBytes = SMEM; cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = S; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    count_launch();
-    return cudaLaunchKernelEx(&cfg, kern, *tmA, *tmB, M, K, ep);
+    return launch_gemm_kernel<gemm_clusterk_kernel<S, D>>(LaunchGrid(dim3(n_tiles * S), S), CkCfg<S>::SMEM_BYTES, stream, *tmA, *tmB, M, K, ep);
 }
 
 template <int D>
@@ -237,19 +164,19 @@ static cudaError_t launch_ck_s(int S, const CUtensorMap* tmA, const CUtensorMap*
 // cluster size for an N x K projection on `sms` SMs: the largest of {8, 4, 3, 2} with n_tiles * S <= sms and >= 2 k-blocks per CTA
 // (0: not worth it — fewer than min_fill_pct % of the SMs would stream)
 int clusterk_pick(int N, int K, int sms, int min_fill_pct) {
-    const int n_tiles = (N + CK_BN - 1) / CK_BN, kb = (K + CK_BK - 1) / CK_BK;
+    const int n_tiles = (N + CK_BN - 1) / CK_BN, kb = (K + BLOCK_K - 1) / BLOCK_K;
     for (int S : {8, 4, 3, 2})
         if (n_tiles * S <= sms && kb >= 2 * S) return (n_tiles * S * 100 >= sms * min_fill_pct) ? S : 0;
     return 0;
 }
 
 cudaError_t launch_gemm_clusterk_resid(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, int S, void* x, int ldx, cudaStream_t stream) {
-    if (M <= 0 || M > CK_BM || (N % 8) != 0 || (K % 8) != 0 || !x || (ldx % 8) != 0) return cudaErrorInvalidValue;
+    if (M <= 0 || M > BLOCK_M || (N % 8) != 0 || (K % 8) != 0 || !x || (ldx % 8) != 0) return cudaErrorInvalidValue;
     CkEpi ep{}; ep.kind = 2; ep.x = reinterpret_cast<uint16_t*>(x); ep.ldx = ldx; ep.N = N;
     return launch_ck_s<128>(S, tmA, tmB, M, N, K, ep, stream);          // D only fixes the unit pairing: any pairing suits the residual epilogue
 }
 cudaError_t launch_gemm_clusterk_rope(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, int S, const SkRopeArgs& rope, cudaStream_t stream) {
-    if (M <= 0 || M > CK_BM || (K % 8) != 0 || N != (rope.nh + 2 * rope.nkv) * rope.D) return cudaErrorInvalidValue;
+    if (M <= 0 || M > BLOCK_M || (K % 8) != 0 || N != (rope.nh + 2 * rope.nkv) * rope.D) return cudaErrorInvalidValue;
     CkEpi ep{}; ep.kind = 3; ep.N = N; ep.rope = rope;
     if (rope.D == 128) return launch_ck_s<128>(S, tmA, tmB, M, N, K, ep, stream);
     if (rope.D == 64) return launch_ck_s<64>(S, tmA, tmB, M, N, K, ep, stream);

@@ -14,7 +14,7 @@ namespace oa {
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
                       uint32_t box_rows, uint32_t box_cols);
 
-// ---- GEMM (gemm_tcgen05.cu): C[M,N] = A[M,K] . B[N,K]^T, bf16 in, fp32 accumulate in registers ----
+// ---- GEMM (gemm_wgmma.cu): C[M,N] = A[M,K] . B[N,K]^T, bf16 in, fp32 accumulate in registers ----
 enum GemmEpilogue : int {
     EPI_STORE = 0,    // out[M,N] bf16 = acc (+ bias[N])
     EPI_RESID = 1,    // out[M,N] bf16 = acc + resid[M,N]      (out may alias resid)
@@ -68,10 +68,6 @@ cudaError_t launch_sk_resid_rmsnorm(const StreamK& sk, void* x, const void* gain
 // act[T,F] = silu(gate) * up from the interleaved gate/up partials (N = 2F)
 cudaError_t launch_sk_swiglu(const StreamK& sk, void* act, int T, int F, cudaStream_t s);
 
-// ---- chained decode kernel: up to 4 stream-K GEMMs and their consumers in ONE persistent launch (gemm_tcgen05.cu) ----
-// Phase p = GEMM p (fp32 partials into the shared workspace) -> grid barrier -> consumer p on all CTAs -> grid barrier -> GEMM p+1
-// (whose weight tiles are already streaming).  Same partial layout, reduction order and consumer code as the stand-alone
-// kernels, so results are bit-identical to launching them one by one.
 struct SkRopeArgs {       // q/k/v from the qkv projection's partials (+ bias): sum -> bf16 -> RoPE -> bf16 (the oracle's order)
     const uint16_t* bias; const int32_t* positions; const int32_t* slots; const float* rope_cos; const float* rope_sin;
     uint16_t* q_out; uint16_t* kv_base; int64_t k_plane_row0, v_plane_row0; int32_t page_size, nh, nkv, D;
@@ -181,15 +177,29 @@ inline cudaError_t ensure_dynamic_smem(K kern, int bytes, bool (&done)[16]) {
     return cudaSuccess;
 }
 
+// A launch grid, optionally of thread-block clusters of `cluster` CTAs along x (a dim3 converts to a grid without clusters).
+struct LaunchGrid {
+    dim3 dim; unsigned cluster;
+    LaunchGrid(dim3 d, unsigned cluster_x = 1) : dim(d), cluster(cluster_x) {}
+};
 // Every kernel launch goes through here: counts it and (unless OA_PDL=0) marks it for programmatic dependent launch.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_k(void (*kern)(KArgs...), LaunchGrid grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.gridDim = grid.dim; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[2];
+    unsigned n = 0;
+    if (grid.cluster > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = grid.cluster; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
+        ++n;
+    }
+    if (pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    cfg.attrs = attr; cfg.numAttrs = n;
     count_launch();
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }

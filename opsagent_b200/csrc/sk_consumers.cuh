@@ -1,6 +1,7 @@
 // sk_consumers.cuh — the consumers of stream-K partials as device functions: each adds a tile's fp32 partials in CTA
-// order (deterministic) and finishes the op.  Shared by the stand-alone consumer kernels (elementwise.cu) and by the
-// GEMM epilogues that finish an op themselves (gemm_tcgen05.cu FUSE=2/3, gemm_clusterk.cu), so every path produces bit-identical results.
+// order (deterministic) and finishes the op with the bf16x8 epilogue helpers of common.cuh.  The stand-alone consumer kernels
+// (elementwise.cu, tp_comm.cu) run these functions; the GEMM epilogues that finish an op themselves (gemm_wgmma.cu FUSE=1/2/3,
+// gemm_clusterk.cu) sum in the same order and call the same helpers and rope_dst_row, so every path produces bit-identical results.
 #pragma once
 #include "common.cuh"
 #include "kernels.hpp"
@@ -94,14 +95,12 @@ OA_DEVINL void sk_resid_rmsnorm_row(const StreamK& sk, int t, int tid, float* re
             if constexpr (SUM) {
                 float acc[8];
                 sk_sum8(sk, t, i * 8, acc);
-                xn.x = pack_bf16x2(bf16lo(xo.x) + acc[0], bf16hi(xo.x) + acc[1]); xn.y = pack_bf16x2(bf16lo(xo.y) + acc[2], bf16hi(xo.y) + acc[3]);
-                xn.z = pack_bf16x2(bf16lo(xo.z) + acc[4], bf16hi(xo.z) + acc[5]); xn.w = pack_bf16x2(bf16lo(xo.w) + acc[6], bf16hi(xo.w) + acc[7]);
+                add_bf16x8(acc, xo);
+                xn = pack_bf16x8(acc);
                 xr[i] = xn;
             }
             v[k] = xn;
-            float a;
-            a = bf16lo(xn.x); ss += a * a; a = bf16hi(xn.x); ss += a * a; a = bf16lo(xn.y); ss += a * a; a = bf16hi(xn.y); ss += a * a;
-            a = bf16lo(xn.z); ss += a * a; a = bf16hi(xn.z); ss += a * a; a = bf16lo(xn.w); ss += a * a; a = bf16hi(xn.w); ss += a * a;
+            ss = sumsq_bf16x8(xn, ss);
         }
     }
     ss = warp_sum(ss);
@@ -115,14 +114,7 @@ OA_DEVINL void sk_resid_rmsnorm_row(const StreamK& sk, int t, int tid, float* re
 #pragma unroll
     for (int k = 0; k < VPT; ++k) {
         const int i = tid + k * SK_RESID_THREADS;
-        if (i < H8) {
-            uint4 o;
-            o.x = pack_bf16x2(bf16lo(v[k].x) * r * bf16lo(gg[k].x), bf16hi(v[k].x) * r * bf16hi(gg[k].x));
-            o.y = pack_bf16x2(bf16lo(v[k].y) * r * bf16lo(gg[k].y), bf16hi(v[k].y) * r * bf16hi(gg[k].y));
-            o.z = pack_bf16x2(bf16lo(v[k].z) * r * bf16lo(gg[k].z), bf16hi(v[k].z) * r * bf16hi(gg[k].z));
-            o.w = pack_bf16x2(bf16lo(v[k].w) * r * bf16lo(gg[k].w), bf16hi(v[k].w) * r * bf16hi(gg[k].w));
-            yr[i] = o;
-        }
+        if (i < H8) yr[i] = rms_scale_bf16x8(v[k], r, gg[k]);
     }
 }
 
@@ -132,33 +124,20 @@ OA_DEVINL void sk_swiglu_item(const StreamK& sk, int t, int i, uint4* __restrict
     float gt[8], up[8];
     sk_sum8(sk, t, blk * 32 + o, gt);
     sk_sum8(sk, t, blk * 32 + 16 + o, up);
-    float f[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) f[k] = __fdividef(gt[k], 1.0f + __expf(-gt[k])) * up[k];
-    uint4 ov;
-    ov.x = pack_bf16x2(f[0], f[1]); ov.y = pack_bf16x2(f[2], f[3]); ov.z = pack_bf16x2(f[4], f[5]); ov.w = pack_bf16x2(f[6], f[7]);
-    act[(size_t)t * F8 + i] = ov;
+    act[(size_t)t * F8 + i] = swiglu_bf16x8(gt, up);
 }
 
-// + bias, then round: the projection output is a bf16 tensor
-OA_DEVINL void sk_finish8_bf16(const uint16_t* bias, int col, float (&v)[8]) {
-    if (bias) {
-        const uint4 bb = *reinterpret_cast<const uint4*>(bias + col);
-        v[0] += bf16lo(bb.x); v[1] += bf16hi(bb.x); v[2] += bf16lo(bb.y); v[3] += bf16hi(bb.y);
-        v[4] += bf16lo(bb.z); v[5] += bf16hi(bb.z); v[6] += bf16lo(bb.w); v[7] += bf16hi(bb.w);
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = bf16_bits_to_f32(f32_to_bf16_bits(v[k]));
+// summed qkv columns [col, col + 8) + bias, then rounded: the projection output is a bf16 tensor
+OA_DEVINL void qkv_finish8(const uint16_t* bias, int col, float* v) {
+    if (bias) add_bf16x8(v, *reinterpret_cast<const uint4*>(bias + col));
+    round_bf16x8(v);
 }
-OA_DEVINL void sk_load8_bf16(const StreamK& sk, const uint16_t* bias, int row, int col, float (&v)[8]) {
-    sk_sum8(sk, row, col, v);
-    if (bias) {
-        const uint4 bb = *reinterpret_cast<const uint4*>(bias + col);
-        v[0] += bf16lo(bb.x); v[1] += bf16hi(bb.x); v[2] += bf16lo(bb.y); v[3] += bf16hi(bb.y);
-        v[4] += bf16lo(bb.z); v[5] += bf16hi(bb.z); v[6] += bf16lo(bb.w); v[7] += bf16hi(bb.w);
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = bf16_bits_to_f32(f32_to_bf16_bits(v[k]));     // the projection output is a bf16 tensor
+
+// destination row of q / k / v head `head` (in qkv column order) of token row t: q_out, or the paged K / V plane at (page, off)
+OA_DEVINL uint16_t* rope_dst_row(const SkRopeArgs& a, int t, int head, int page, int off) {
+    if (head < a.nh) return a.q_out + (size_t)t * a.nh * a.D + (size_t)head * a.D;
+    if (head < a.nh + a.nkv) return kv_row(a.kv_base, a.k_plane_row0, page, a.nkv, head - a.nh, a.page_size, off, a.D);
+    return kv_row(a.kv_base, a.v_plane_row0, page, a.nkv, head - a.nh - a.nkv, a.page_size, off, a.D);
 }
 
 OA_DEVINL int sk_rope_items_per_row(const SkRopeArgs& a) { return (a.nh + a.nkv) * (a.D >> 4) + a.nkv * (a.D >> 3); }
@@ -170,37 +149,21 @@ OA_DEVINL void sk_rope_item(const StreamK& sk, const SkRopeArgs& a, int t, int w
     const int n_rot = (a.nh + a.nkv) * vec_per_head;
     if (w < n_rot) {
         const int pos = a.positions[t];
-        const float* cr = a.rope_cos + (size_t)pos * half;
-        const float* sr = a.rope_sin + (size_t)pos * half;
         const int head = w / vec_per_head, i0 = (w - head * vec_per_head) * 8;
         float av[8], bv[8];
         sk_sum8_pair(sk, t, head * D + i0, head * D + i0 + half, av, bv);
-        sk_finish8_bf16(a.bias, head * D + i0, av);
-        sk_finish8_bf16(a.bias, head * D + i0 + half, bv);
-        const float4 c0 = *reinterpret_cast<const float4*>(cr + i0), c1 = *reinterpret_cast<const float4*>(cr + i0 + 4);
-        const float4 s0 = *reinterpret_cast<const float4*>(sr + i0), s1 = *reinterpret_cast<const float4*>(sr + i0 + 4);
-        const float cv[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-        const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-        float ra[8], rb[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) { ra[k] = av[k] * cv[k] - bv[k] * sv[k]; rb[k] = bv[k] * cv[k] + av[k] * sv[k]; }
-        uint4 oa, ob;
-        oa.x = pack_bf16x2(ra[0], ra[1]); oa.y = pack_bf16x2(ra[2], ra[3]); oa.z = pack_bf16x2(ra[4], ra[5]); oa.w = pack_bf16x2(ra[6], ra[7]);
-        ob.x = pack_bf16x2(rb[0], rb[1]); ob.y = pack_bf16x2(rb[2], rb[3]); ob.z = pack_bf16x2(rb[4], rb[5]); ob.w = pack_bf16x2(rb[6], rb[7]);
-        uint16_t* dst;
-        if (head < a.nh) dst = a.q_out + (size_t)t * a.nh * D + (size_t)head * D;
-        else dst = a.kv_base + (size_t)(a.k_plane_row0 + ((int64_t)page * a.nkv + (head - a.nh)) * a.page_size + off) * D;
-        *reinterpret_cast<uint4*>(dst + i0) = oa;
-        *reinterpret_cast<uint4*>(dst + i0 + half) = ob;
+        qkv_finish8(a.bias, head * D + i0, av);
+        qkv_finish8(a.bias, head * D + i0 + half, bv);
+        uint16_t* dst = rope_dst_row(a, t, head, page, off);
+        rope_bf16x8(av, bv, a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0,
+                    *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
     } else {
         const int wv = w - n_rot;
-        const int head = wv / (D >> 3), i0 = (wv - head * (D >> 3)) * 8;
+        const int head = a.nh + a.nkv + wv / (D >> 3), i0 = (wv % (D >> 3)) * 8;
         float vv[8];
-        sk_load8_bf16(sk, a.bias, t, (a.nh + a.nkv + head) * D + i0, vv);
-        uint4 o;
-        o.x = pack_bf16x2(vv[0], vv[1]); o.y = pack_bf16x2(vv[2], vv[3]); o.z = pack_bf16x2(vv[4], vv[5]); o.w = pack_bf16x2(vv[6], vv[7]);
-        uint16_t* dst = a.kv_base + (size_t)(a.v_plane_row0 + ((int64_t)page * a.nkv + head) * a.page_size + off) * D;
-        *reinterpret_cast<uint4*>(dst + i0) = o;
+        sk_sum8(sk, t, head * D + i0, vv);
+        qkv_finish8(a.bias, head * D + i0, vv);
+        *reinterpret_cast<uint4*>(rope_dst_row(a, t, head, page, off) + i0) = pack_bf16x8(vv);
     }
 }
 

@@ -5,7 +5,7 @@
 // computed by a depth-first walk of a byte trie of the vocabulary — a rejected byte prunes every token below it, so literal states
 // (one allowed byte) cost microseconds and string states visit only the printable-ASCII part of the trie — and cached per
 // (grammar, canonical state).  The bitset [ceil(vocab/32)] goes to the device once per state; the LM-head epilogue of the GEMM
-// applies it while it computes the row arg-max (gemm_tcgen05.cu EPI_LOGITS), so constrained rows cost no extra kernel.
+// applies it while it computes the row arg-max (gemm_wgmma.cu EPI_LOGITS), so constrained rows cost no extra kernel.
 // This is what lets `json_mode` / OpenAI function calling work on real checkpoints (reference consumer: pkg/assistants/simple.go:366-382
 // json.Unmarshal into tools.ToolPrompt, pkg/tools/tool.go:29-38).  oracle/oracle.py restates the rule by brute force for the tests.
 #pragma once

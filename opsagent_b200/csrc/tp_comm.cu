@@ -442,10 +442,8 @@ __global__ void ar_resid_bf16_kernel(const uint16_t* const* __restrict__ peer, i
             acc[0] += bf16lo(a[p].x); acc[1] += bf16hi(a[p].x); acc[2] += bf16lo(a[p].y); acc[3] += bf16hi(a[p].y);
             acc[4] += bf16lo(a[p].z); acc[5] += bf16hi(a[p].z); acc[6] += bf16lo(a[p].w); acc[7] += bf16hi(a[p].w);
         }
-        const uint4 xo = x[i]; uint4 xn;
-        xn.x = pack_bf16x2(bf16lo(xo.x) + acc[0], bf16hi(xo.x) + acc[1]); xn.y = pack_bf16x2(bf16lo(xo.y) + acc[2], bf16hi(xo.y) + acc[3]);
-        xn.z = pack_bf16x2(bf16lo(xo.z) + acc[4], bf16hi(xo.z) + acc[5]); xn.w = pack_bf16x2(bf16lo(xo.w) + acc[6], bf16hi(xo.w) + acc[7]);
-        x[i] = xn;
+        add_bf16x8(acc, x[i]);
+        x[i] = pack_bf16x8(acc);
     }
 }
 cudaError_t launch_ar_resid_bf16(void* const* d_peer, int t, void* x, int T, int H, cudaStream_t s) {
@@ -471,9 +469,8 @@ __global__ void ar2_reduce_scatter_kernel(const uint16_t* const* __restrict__ pe
             acc[0] += bf16lo(a[p].x); acc[1] += bf16hi(a[p].x); acc[2] += bf16lo(a[p].y); acc[3] += bf16hi(a[p].y);
             acc[4] += bf16lo(a[p].z); acc[5] += bf16hi(a[p].z); acc[6] += bf16lo(a[p].w); acc[7] += bf16hi(a[p].w);
         }
-        const uint4 xo = x[i]; uint4 xn;
-        xn.x = pack_bf16x2(bf16lo(xo.x) + acc[0], bf16hi(xo.x) + acc[1]); xn.y = pack_bf16x2(bf16lo(xo.y) + acc[2], bf16hi(xo.y) + acc[3]);
-        xn.z = pack_bf16x2(bf16lo(xo.z) + acc[4], bf16hi(xo.z) + acc[5]); xn.w = pack_bf16x2(bf16lo(xo.w) + acc[6], bf16hi(xo.w) + acc[7]);
+        add_bf16x8(acc, x[i]);
+        const uint4 xn = pack_bf16x8(acc);
         x[i] = xn; gather[i] = xn;
     }
 }
@@ -538,23 +535,9 @@ struct ValIdx { float v; int i; };
 __global__ void argmax_reduce_pair_kernel(const float* __restrict__ val, const int* __restrict__ idx, int n_tiles, int idx_offset, ValIdx* __restrict__ out) {
     griddep_launch(); griddep_wait();
     const int row = blockIdx.x;
-    float bv = -INFINITY; int bi = 0x7fffffff;
-    for (int t = threadIdx.x; t < n_tiles; t += blockDim.x) {
-        const float v = val[(size_t)row * n_tiles + t]; const int i = idx[(size_t)row * n_tiles + t];
-        if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    __shared__ float sv[8]; __shared__ int si[8];
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = bv; si[threadIdx.x >> 5] = bi; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) if (sv[w] > bv || (sv[w] == bv && si[w] < bi)) { bv = sv[w]; bi = si[w]; }
-        out[row].v = bv; out[row].i = (bi == 0x7fffffff ? 0 : bi) + idx_offset;
-    }
+    float bv; int bi;
+    block_argmax_row(val, idx, row, n_tiles, bv, bi);
+    if (threadIdx.x == 0) { out[row].v = bv; out[row].i = (bi == 0x7fffffff ? 0 : bi) + idx_offset; }
 }
 cudaError_t launch_argmax_reduce_pair(const float* amax_val, const int* amax_idx, int M, int n_tiles, int idx_offset, void* pair_out, cudaStream_t s) {
     return launch_k(argmax_reduce_pair_kernel, dim3(M), dim3(256), 0, s, amax_val, amax_idx, n_tiles, idx_offset, reinterpret_cast<ValIdx*>(pair_out));
