@@ -73,7 +73,8 @@ typedef struct {
 } oa_chat_resp;
 
 /* config_json: {"model":"llama-3-8b"|"llama-3.2-1b"|"qwen2.5-32b"|"llama-3-70b"|custom dims..., "seed":1234,
- *  "device":0, "kv_gb":100, "max_batch":128, "max_seq_len":4096, "max_step_tokens":8192, ...} — see DESIGN.md */
+ *  "device":0, "kv_gb":100, "max_batch":128, "max_seq_len":4096, "max_step_tokens":8192,
+ *  "kv_cache_dtype":"bf16"|"fp8_e4m3", ...} — see DESIGN.md */
 OA_API int oa_engine_create(const char* config_json, oa_engine** out);
 OA_API void oa_engine_destroy(oa_engine*);
 /* tensor-parallel groups (config "tp": t, "tp_rank": r, "tp_shm": name; one process per GPU): rank 0 is the engine callers talk
@@ -145,6 +146,16 @@ OA_API int oa_k_init_weight(void* dst, uint64_t seed, uint64_t tensor_id, int64_
 OA_API int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
                          int32_t max_pages_per_seq, const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs,
                          int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t force_splits, void* stream);
+/* the same on an fp8 (e4m3) cache of the same shape in bytes, each (page, kv head) block holding K as [64][D] and V transposed as [D][64];
+ * K bytes decode to e4m3 * k_scale, V bytes to e4m3 * v_scale */
+OA_API int oa_k_paged_attention_fp8(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
+                             int32_t max_pages_per_seq, const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs,
+                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t force_splits, float k_scale, float v_scale, void* stream);
+/* the engine's RoPE + KV write (one layer) into such a cache: qkv [T, (n_heads + 2 n_kv) * D] bf16, positions / slots [T] and the RoPE
+ * tables (fp32 [positions][D/2]) on the device; rotated q -> q_out [T, n_heads * D] */
+OA_API int oa_k_kv_write_fp8(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos, const float* rope_sin,
+                      void* q_out, void* kv_cache, int32_t num_pages, int32_t T, int32_t n_heads, int32_t n_kv, int32_t head_dim,
+                      float k_scale, float v_scale, void* stream);
 /* ---- host-only logic, callable without a GPU (CPU tests) ---- */
 /* chat template + tokenizer of the model described by config_json */
 OA_API int oa_host_apply_chat_template(const char* config_json, const oa_msg* msgs, int32_t n_msgs, int32_t* out_ids, int32_t cap, int32_t* n_out);

@@ -37,6 +37,22 @@ struct AttCfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + SCRATCH_BYTES + 4 * 8 * 2 * 4 + 2 * STAGES * 8 + 1024;
 };
 
+// fp8 cache (KvLayout::fp8): a (page, kv head) block is 64 * D bytes, K as [64 tokens][D] and V as [D][64 tokens].  TMA reads the pool as
+// rows of 128 bytes (make_tmap_u8_2d, box {128, D/2}: one block per load) with the 128-byte swizzle, so byte o of a staged block
+// sits at fp8_swz(o).  Decode builds its mma operands straight from these bytes; prefill widens each stage to bf16 first.
+template <int D, bool FP8>
+struct DecCfg {
+    static constexpr int KV_BYTES = FP8 ? PAGE * D : AttCfg<D>::KV_BYTES;
+    static constexpr int STAGE_BYTES = 2 * KV_BYTES;
+    static constexpr int STAGES = FP8 ? 2 * AttCfg<D>::STAGES : AttCfg<D>::STAGES;     // same bytes in flight per SM
+    static constexpr int SCRATCH_BYTES = AttCfg<D>::SCRATCH_BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + SCRATCH_BYTES + 4 * 8 * 2 * 4 + 2 * STAGES * 8 + 1024;
+};
+OA_DEVINL uint32_t fp8_swz(uint32_t o) { return o ^ (((o >> 7) & 7u) << 4); }
+// row of the pool's 128-byte view where the fp8 block starting at token row `row` (KvLayout rows of D elements) begins
+template <int D>
+OA_DEVINL int32_t fp8_tma_row(int64_t row) { return (int32_t)(row * D / 128); }
+
 // byte offset of the 16-byte chunk holding (row r, columns d..d+7) inside one K or V stage buffer
 template <int D>
 OA_DEVINL uint32_t kv_off(int r, int d) {
@@ -48,11 +64,15 @@ OA_DEVINL void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" :
 // =============================================================================================
 // decode
 // =============================================================================================
-template <int D>
+// FP8: K / V bytes of the fp8 cache.  The token order inside a warp's 16-token quarter is permuted so that both products read their fp8
+// operand along its reduction dimension with plain ldmatrix: S column 2t+e of n-tile j is token 4t+2j+e, and the head dims of each
+// 16-wide k-step are paired (4t, 4t+1) / (4t+2, 4t+3) in Q and K alike.  P's fragment then holds tokens 4t..4t+3, which is what an
+// ldmatrix row of the transposed V block gives.  k_scale is in p.scale_log2e; v_scale multiplies the output.
+template <int D, bool FP8>
 __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const __grid_constant__ CUtensorMap tm_kv,
                                                                           const DecodeAttnParams p, const int64_t layer_row0,
-                                                                          const int64_t kv_stride_rows) {
-    using Cfg = AttCfg<D>;
+                                                                          const int64_t kv_stride_rows, const float v_scale) {
+    using Cfg = DecCfg<D, FP8>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int KS = D / 16;      // k-steps of Q·K^T
     constexpr int NT = D / 8;       // n-tiles of P·V
@@ -97,10 +117,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                     mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
                     const int64_t krow = layer_row0 + ((int64_t)page * p.n_kv + sg.kvh) * PAGE;
                     const int64_t vrow = krow + kv_stride_rows;
+                    if constexpr (FP8) {
+                        tma_load_2d(kdst, &tm_kv, &full_bar[s], 0, fp8_tma_row<D>(krow), kEvictFirst);
+                        tma_load_2d(vdst, &tm_kv, &full_bar[s], 0, fp8_tma_row<D>(vrow), kEvictFirst);
+                    } else {
 #pragma unroll
-                    for (int h = 0; h < Cfg::HALVES; ++h) {
-                        tma_load_2d(kdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)krow, kEvictFirst);
-                        tma_load_2d(vdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)vrow, kEvictFirst);
+                        for (int h = 0; h < AttCfg<D>::HALVES; ++h) {
+                            tma_load_2d(kdst + h * AttCfg<D>::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)krow, kEvictFirst);
+                            tma_load_2d(vdst + h * AttCfg<D>::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)vrow, kEvictFirst);
+                        }
                     }
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
@@ -123,8 +148,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
 #pragma unroll
             for (int ks = 0; ks < KS; ++ks) {
                 if (g < grp) {
-                    qa[ks][0] = *reinterpret_cast<const uint32_t*>(qrow + ks * 16 + 2 * t);
-                    qa[ks][1] = *reinterpret_cast<const uint32_t*>(qrow + ks * 16 + 8 + 2 * t);
+                    const int d0 = FP8 ? 4 * t : 2 * t, d1 = FP8 ? 4 * t + 2 : 8 + 2 * t;
+                    qa[ks][0] = *reinterpret_cast<const uint32_t*>(qrow + ks * 16 + d0);
+                    qa[ks][1] = *reinterpret_cast<const uint32_t*>(qrow + ks * 16 + d1);
                 } else { qa[ks][0] = 0u; qa[ks][1] = 0u; }
             }
         }
@@ -142,7 +168,21 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                 float sacc[2][4];
 #pragma unroll
                 for (int j = 0; j < 2; ++j) { sacc[j][0] = sacc[j][1] = sacc[j][2] = sacc[j][3] = 0.f; }
-                {
+                if constexpr (FP8) {
+                    // matrix m = lane / 8 of each ldmatrix.x4: n-tile m & 1, k-step 2kk + (m >> 1); its row c = lane % 8 is token 4(c/2) + 2(m&1) + c%2
+                    const int m = lane >> 3, c = lane & 7;
+                    const uint32_t row0 = (uint32_t)(warp * 16 + 4 * (c >> 1) + 2 * (m & 1) + (c & 1)) * D + (uint32_t)(m >> 1) * 16;
+#pragma unroll
+                    for (int kk = 0; kk < KS / 2; ++kk) {
+                        uint32_t r[4];
+                        ldmatrix_x4(kbase + fp8_swz(row0 + kk * 32), r[0], r[1], r[2], r[3]);
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int ks = 2 * kk + (i >> 1);
+                            mma_bf16_16816(sacc[i & 1], qa[ks][0], 0u, qa[ks][1], 0u, e4m3x2_to_bf16x2((uint16_t)r[i]), e4m3x2_to_bf16x2((uint16_t)(r[i] >> 16)));
+                        }
+                    }
+                } else {
                     const int r = warp * 16 + ((lane >> 4) << 3) + (lane & 7);
                     const int dsel = ((lane >> 3) & 1) << 3;
 #pragma unroll
@@ -159,7 +199,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                 for (int j = 0; j < 2; ++j)
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        const int tok = tok0 + j * 8 + 2 * t + e;
+                        const int tok = tok0 + (FP8 ? 4 * t + 2 * j : j * 8 + 2 * t) + e;
                         sc[j * 2 + e] = tok < ctx ? sacc[j][e] * p.scale_log2e : -INFINITY;
                     }
                 float mx = fmaxf(fmaxf(sc[0], sc[1]), fmaxf(sc[2], sc[3]));
@@ -173,7 +213,20 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                 l_run = l_run * alpha + (pr[0] + pr[1] + pr[2] + pr[3]);
                 m_run = m_new;
                 const uint32_t pa0 = pack_bf16x2(pr[0], pr[1]), pa2 = pack_bf16x2(pr[2], pr[3]);
-                {
+                if constexpr (FP8) {
+                    // matrix m of ldmatrix.x4 number jj: n-tile 4jj + m, rows = its 8 head dims, 16 bytes = this warp's 16 tokens
+                    const uint32_t row0 = (uint32_t)(8 * (lane >> 3) + (lane & 7)) * PAGE + warp * 16;
+#pragma unroll
+                    for (int j = 0; j < NT; ++j) { oacc[j][0] *= alpha; oacc[j][1] *= alpha; }
+#pragma unroll
+                    for (int jj = 0; jj < NT / 4; ++jj) {
+                        uint32_t r[4];
+                        ldmatrix_x4(vbase + fp8_swz(row0 + jj * 32 * PAGE), r[0], r[1], r[2], r[3]);
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+                            mma_bf16_16816(oacc[4 * jj + i], pa0, 0u, pa2, 0u, e4m3x2_to_bf16x2((uint16_t)r[i]), e4m3x2_to_bf16x2((uint16_t)(r[i] >> 16)));
+                    }
+                } else {
                     const int r = warp * 16 + (((lane >> 3) & 1) << 3) + (lane & 7);
                     const int dsel = (lane >> 4) << 3;
 #pragma unroll
@@ -220,7 +273,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                 }
             if (g < grp) {
                 if (sg.partial_slot < 0) {
-                    const float inv = 1.0f / l_tot;
+                    const float inv = (FP8 ? v_scale : 1.0f) / l_tot;
                     uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (size_t)sg.seq * p.n_heads * D + (size_t)(sg.kvh * grp + g) * D;
 #pragma unroll
                     for (int j = 0; j < NT; ++j)
@@ -228,7 +281,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) decode_attention_kernel(const 
                 } else {
                     float* po = p.part_o + ((size_t)sg.partial_slot * grp + g) * D;
 #pragma unroll
-                    for (int j = 0; j < NT; ++j) *reinterpret_cast<float2*>(po + j * 8 + 2 * t) = make_float2(oacc[j][0], oacc[j][1]);
+                    for (int j = 0; j < NT; ++j) {
+                        if constexpr (FP8) *reinterpret_cast<float2*>(po + j * 8 + 2 * t) = make_float2(oacc[j][0] * v_scale, oacc[j][1] * v_scale);
+                        else *reinterpret_cast<float2*>(po + j * 8 + 2 * t) = make_float2(oacc[j][0], oacc[j][1]);
+                    }
                     if (t == 0) {
                         p.part_ml[((size_t)sg.partial_slot * grp + g) * 2] = m_tot;
                         p.part_ml[((size_t)sg.partial_slot * grp + g) * 2 + 1] = l_tot;
@@ -299,19 +355,23 @@ cudaError_t launch_decode_merge(const MergeItem* items, int n_items, const float
     return launch_k(decode_merge_kernel, dim3(n_items), dim3(128), 0, s, items, part_o, part_ml, reinterpret_cast<uint16_t*>(out), n_heads, n_kv, head_dim);
 }
 
-template <int D>
+template <int D, bool FP8>
 static cudaError_t launch_decode_d(const CUtensorMap* tm_kv, const KvLayout& kv, const DecodeAttnParams& p, cudaStream_t s) {
-    auto kern = decode_attention_kernel<D>;
+    auto kern = decode_attention_kernel<D, FP8>;
+    constexpr int SMEM = DecCfg<D, FP8>::SMEM_BYTES;
     static bool attr_done[16] = {};
-    { cudaError_t e = ensure_dynamic_smem(kern, AttCfg<D>::SMEM_BYTES, attr_done); if (e != cudaSuccess) return e; }
-    return launch_k(kern, dim3(p.n_ctas), dim3(ATT_THREADS), AttCfg<D>::SMEM_BYTES, s, *tm_kv, p, (int64_t)p.layer * kv.layer_stride_rows, kv.kv_stride_rows);
+    { cudaError_t e = ensure_dynamic_smem(kern, SMEM, attr_done); if (e != cudaSuccess) return e; }
+    DecodeAttnParams q = p;
+    float v_scale = 1.0f;
+    if (FP8) { q.scale_log2e = p.scale_log2e * kv.k_scale[p.layer]; v_scale = kv.v_scale[p.layer]; }
+    return launch_k(kern, dim3(p.n_ctas), dim3(ATT_THREADS), SMEM, s, *tm_kv, q, (int64_t)p.layer * kv.layer_stride_rows, kv.kv_stride_rows, v_scale);
 }
 
 cudaError_t launch_decode_attention(const CUtensorMap* tm_kv, const KvLayout& kv, const DecodeAttnParams& p, cudaStream_t s) {
     if (p.n_ctas <= 0) return cudaSuccess;
     if (kv.page_size != PAGE || p.n_heads % p.n_kv != 0 || p.n_heads / p.n_kv > 8) return cudaErrorInvalidValue;
-    if (kv.head_dim == 128) return launch_decode_d<128>(tm_kv, kv, p, s);
-    if (kv.head_dim == 64) return launch_decode_d<64>(tm_kv, kv, p, s);
+    if (kv.head_dim == 128) return kv.fp8 ? launch_decode_d<128, true>(tm_kv, kv, p, s) : launch_decode_d<128, false>(tm_kv, kv, p, s);
+    if (kv.head_dim == 64) return kv.fp8 ? launch_decode_d<64, true>(tm_kv, kv, p, s) : launch_decode_d<64, false>(tm_kv, kv, p, s);
     return cudaErrorInvalidValue;
 }
 
@@ -321,19 +381,60 @@ cudaError_t launch_decode_attention(const CUtensorMap* tm_kv, const KvLayout& kv
 static constexpr int PREFILL_WARPS = PREFILL_TILE_ROWS / 16;            // 8 consumer warps x 16 query rows share every K/V stage
 static constexpr int PREFILL_THREADS = (PREFILL_WARPS + 1) * 32;        // + 1 TMA producer warp
 
+template <int D, bool FP8>
+struct PreCfg {
+    static constexpr int RING_BYTES = FP8 ? 2 * PAGE * D : AttCfg<D>::STAGE_BYTES;        // one TMA stage (K and V of one page)
+    static constexpr int STAGES = FP8 ? 4 : AttCfg<D>::STAGES;
+    static constexpr int WIDE_BYTES = FP8 ? 2 * AttCfg<D>::STAGE_BYTES : 0;               // fp8: two bf16 copies of a stage (double buffer)
+    static constexpr int SMEM_BYTES = STAGES * RING_BYTES + WIDE_BYTES + 2 * STAGES * 8 + 1024;
+};
+
+// fp8 prefill: the consumer warps widen a staged page to bf16 before the wgmma products read it.  K [64][D] bytes -> the bf16 K tile layout
+// (kv_off); V [D][64] bytes -> D rows of 64 bf16 tokens with the 128-byte swizzle, i.e. a K-major B operand of P·V.
+template <int D>
+OA_DEVINL void widen_fp8_stage(const uint8_t* src, uint8_t* dst, int tid) {
+    constexpr int CHUNKS = PAGE * D / 16;          // 16-byte chunks of K (and of V)
+    auto widen16 = [](uint4 b, uint4& lo, uint4& hi) {
+        lo.x = e4m3x2_to_bf16x2((uint16_t)b.x); lo.y = e4m3x2_to_bf16x2((uint16_t)(b.x >> 16));
+        lo.z = e4m3x2_to_bf16x2((uint16_t)b.y); lo.w = e4m3x2_to_bf16x2((uint16_t)(b.y >> 16));
+        hi.x = e4m3x2_to_bf16x2((uint16_t)b.z); hi.y = e4m3x2_to_bf16x2((uint16_t)(b.z >> 16));
+        hi.z = e4m3x2_to_bf16x2((uint16_t)b.w); hi.w = e4m3x2_to_bf16x2((uint16_t)(b.w >> 16));
+    };
+#pragma unroll
+    for (int q = tid; q < CHUNKS; q += PREFILL_WARPS * 32) {
+        const int r = q / (D / 16), d0 = (q % (D / 16)) * 16;
+        uint4 lo, hi;
+        widen16(*reinterpret_cast<const uint4*>(src + fp8_swz((uint32_t)(r * D + d0))), lo, hi);
+        *reinterpret_cast<uint4*>(dst + kv_off<D>(r, d0)) = lo;
+        *reinterpret_cast<uint4*>(dst + kv_off<D>(r, d0 + 8)) = hi;
+    }
+#pragma unroll
+    for (int q = tid; q < CHUNKS; q += PREFILL_WARPS * 32) {
+        const int d = q >> 2, c0 = (q & 3) * 2;        // head dim d, tokens 8 c0 .. 8 c0 + 15
+        uint4 lo, hi;
+        widen16(*reinterpret_cast<const uint4*>(src + PAGE * D + fp8_swz((uint32_t)(d * PAGE + c0 * 8))), lo, hi);
+        uint8_t* row = dst + AttCfg<D>::KV_BYTES + d * 128;
+        *reinterpret_cast<uint4*>(row + ((c0 ^ (d & 7)) << 4)) = lo;
+        *reinterpret_cast<uint4*>(row + (((c0 + 1) ^ (d & 7)) << 4)) = hi;
+    }
+}
+
 // Both products on wgmma: warpgroup g (warps 4g..4g+3) owns query rows [64g, 64g + 64).  S = Q·Kᵀ is m64n64k16 with Q from registers (the mma.sync A-fragment layout) and K K-major as TMA stored it;
 // O += P·V is m64nDk16 with P from registers and V read MN-major (d contiguous, as stored).  The accumulator fragments have the
 // mma.sync C layout (register 4j + e = rows g / g+8, columns 8j + 2t + e), so the online softmax works on them directly.
-template <int D>
+// FP8: pages of the fp8 cache, widened to bf16 per stage (widen_fp8_stage); V is then K-major.  k_scale is in p.scale_log2e.
+template <int D, bool FP8>
 __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(const __grid_constant__ CUtensorMap tm_kv,
                                                                            const PrefillAttnParams p, const int64_t layer_row0,
-                                                                           const int64_t kv_stride_rows) {
+                                                                           const int64_t kv_stride_rows, const float v_scale) {
     using Cfg = AttCfg<D>;
-    constexpr int STAGES = Cfg::STAGES;
+    using PC = PreCfg<D, FP8>;
+    constexpr int STAGES = PC::STAGES;
     constexpr int KS = D / 16, NT = D / 8;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint8_t* wide = smem + STAGES * PC::RING_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(wide + PC::WIDE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -358,15 +459,20 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
             for (int c = 0; c < n_chunks; ++c) {
                 const int page = bt[c];
                 mbar_wait(&empty_bar[s], ph ^ 1);
-                uint8_t* kdst = smem + s * Cfg::STAGE_BYTES;
-                uint8_t* vdst = kdst + Cfg::KV_BYTES;
-                mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+                uint8_t* kdst = smem + s * PC::RING_BYTES;
+                uint8_t* vdst = kdst + PC::RING_BYTES / 2;
+                mbar_expect_tx(&full_bar[s], PC::RING_BYTES);
                 const int64_t krow = layer_row0 + ((int64_t)page * p.n_kv + kvh) * PAGE;
                 const int64_t vrow = krow + kv_stride_rows;
+                if constexpr (FP8) {
+                    tma_load_2d(kdst, &tm_kv, &full_bar[s], 0, fp8_tma_row<D>(krow), kEvictLast);
+                    tma_load_2d(vdst, &tm_kv, &full_bar[s], 0, fp8_tma_row<D>(vrow), kEvictLast);
+                } else {
 #pragma unroll
-                for (int h = 0; h < Cfg::HALVES; ++h) {
-                    tma_load_2d(kdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)krow, kEvictLast);
-                    tma_load_2d(vdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)vrow, kEvictLast);
+                    for (int h = 0; h < Cfg::HALVES; ++h) {
+                        tma_load_2d(kdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)krow, kEvictLast);
+                        tma_load_2d(vdst + h * Cfg::TILE_BYTES, &tm_kv, &full_bar[s], h * 64, (int32_t)vrow, kEvictLast);
+                    }
                 }
                 if (++s == STAGES) { s = 0; ph ^= 1; }
             }
@@ -401,8 +507,18 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
     int s = 0; uint32_t ph = 0;
     for (int c = 0; c < n_chunks; ++c) {
         mbar_wait(&full_bar[s], ph);
+        uint32_t kbase = smem_u32(smem + s * Cfg::STAGE_BYTES);
+        if constexpr (FP8) {
+            // every consumer warp widens its share; the buffer written here was last read for chunk c - 2, which all warps finished
+            // before the barrier of chunk c - 1
+            uint8_t* w = wide + (c & 1) * Cfg::STAGE_BYTES;
+            widen_fp8_stage<D>(smem + s * PC::RING_BYTES, w, threadIdx.x);
+            fence_proxy_async();                    // generic-proxy stores -> wgmma operand reads
+            named_bar_sync(1, PREFILL_WARPS * 32);
+            if (lane == 0) mbar_arrive(&empty_bar[s]);     // every warp has widened its share: the fp8 stage is free for the producer
+            kbase = smem_u32(w);
+        }
         if (c * PAGE <= wg_last_pos) {
-            const uint32_t kbase = smem_u32(smem + s * Cfg::STAGE_BYTES);
             const uint32_t vbase = kbase + Cfg::KV_BYTES;
             float sacc[32];
 #pragma unroll
@@ -448,20 +564,26 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {       // 16 key tokens per step = two 8-row groups of V (1024 B apart)
                 const uint32_t a[4] = {pa[2 * kk][0], pa[2 * kk][1], pa[2 * kk + 1][0], pa[2 * kk + 1][1]};
-                const uint64_t db = gmma_desc_sw128_mn(vbase + (uint32_t)(kk * 2048), (uint32_t)Cfg::TILE_BYTES, 1024u);
-                if constexpr (D == 128) wgmma_rs_m64n128_tb(oacc, a, db, 1u);
-                else wgmma_rs_m64n64_tb(oacc, a, db, 1u);
+                if constexpr (FP8) {                // widened V: D rows of 64 tokens, K-major (+32 B per 16 tokens)
+                    const uint64_t db = gmma_desc_sw128(vbase + (uint32_t)(kk * 32));
+                    if constexpr (D == 128) wgmma_rs_m64n128(oacc, a, db, 1u);
+                    else wgmma_rs_m64n64(oacc, a, db, 1u);
+                } else {
+                    const uint64_t db = gmma_desc_sw128_mn(vbase + (uint32_t)(kk * 2048), (uint32_t)Cfg::TILE_BYTES, 1024u);
+                    if constexpr (D == 128) wgmma_rs_m64n128_tb(oacc, a, db, 1u);
+                    else wgmma_rs_m64n64_tb(oacc, a, db, 1u);
+                }
             }
             wgmma_commit();
             wgmma_wait<0>();                        // V of this stage has been read
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[s]);
+        if (!FP8 && lane == 0) mbar_arrive(&empty_bar[s]);
         if (++s == STAGES) { s = 0; ph ^= 1; }
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+    const float inv0 = (FP8 ? v_scale : 1.0f) / l0, inv1 = (FP8 ? v_scale : 1.0f) / l1;
     uint16_t* ob = reinterpret_cast<uint16_t*>(p.out) + (size_t)head * D;
     const size_t ldo = (size_t)p.n_heads * D;
     if (r0 < tile.n_rows) {
@@ -476,21 +598,24 @@ __global__ void __launch_bounds__(PREFILL_THREADS, 1) prefill_attention_kernel(c
     }
 }
 
-template <int D>
+template <int D, bool FP8>
 static cudaError_t launch_prefill_d(const CUtensorMap* tm_kv, const KvLayout& kv, const PrefillAttnParams& p, cudaStream_t s) {
-    auto kern = prefill_attention_kernel<D>;
-    constexpr int SMEM = AttCfg<D>::STAGES * AttCfg<D>::STAGE_BYTES + 2 * AttCfg<D>::STAGES * 8 + 1024;
+    auto kern = prefill_attention_kernel<D, FP8>;
+    constexpr int SMEM = PreCfg<D, FP8>::SMEM_BYTES;
     static bool attr_done[16] = {};
     { cudaError_t e = ensure_dynamic_smem(kern, SMEM, attr_done); if (e != cudaSuccess) return e; }
     dim3 grid(p.n_tiles, p.n_heads, 1);
-    return launch_k(kern, grid, dim3(PREFILL_THREADS), SMEM, s, *tm_kv, p, (int64_t)p.layer * kv.layer_stride_rows, kv.kv_stride_rows);
+    PrefillAttnParams q = p;
+    float v_scale = 1.0f;
+    if (FP8) { q.scale_log2e = p.scale_log2e * kv.k_scale[p.layer]; v_scale = kv.v_scale[p.layer]; }
+    return launch_k(kern, grid, dim3(PREFILL_THREADS), SMEM, s, *tm_kv, q, (int64_t)p.layer * kv.layer_stride_rows, kv.kv_stride_rows, v_scale);
 }
 
 cudaError_t launch_prefill_attention(const CUtensorMap* tm_kv, const KvLayout& kv, const PrefillAttnParams& p, cudaStream_t s) {
     if (p.n_tiles <= 0) return cudaSuccess;
     if (kv.page_size != PAGE || p.n_heads % p.n_kv != 0) return cudaErrorInvalidValue;
-    if (kv.head_dim == 128) return launch_prefill_d<128>(tm_kv, kv, p, s);
-    if (kv.head_dim == 64) return launch_prefill_d<64>(tm_kv, kv, p, s);
+    if (kv.head_dim == 128) return kv.fp8 ? launch_prefill_d<128, true>(tm_kv, kv, p, s) : launch_prefill_d<128, false>(tm_kv, kv, p, s);
+    if (kv.head_dim == 64) return kv.fp8 ? launch_prefill_d<64, true>(tm_kv, kv, p, s) : launch_prefill_d<64, false>(tm_kv, kv, p, s);
     return cudaErrorInvalidValue;
 }
 

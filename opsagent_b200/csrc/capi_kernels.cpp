@@ -27,6 +27,21 @@ struct DevBuf {
     ~DevBuf() { if (p) cudaFree(p); }
 };
 int rc_of(cudaError_t e) { return e == cudaSuccess ? OA_OK : OA_ERR_INTERNAL; }
+
+// one layer of a paged cache: bf16, or fp8 with the given scales (k_scale / v_scale point at one float each)
+KvLayout one_layer_kv(const void* kv_cache, int32_t num_pages, int32_t n_kv, int32_t head_dim, const float* k_scale, const float* v_scale) {
+    KvLayout kv{}; kv.base = const_cast<void*>(kv_cache); kv.page_size = 64; kv.n_kv = n_kv; kv.head_dim = head_dim; kv.num_pages = num_pages;
+    kv.kv_stride_rows = (int64_t)num_pages * n_kv * 64; kv.layer_stride_rows = 2 * kv.kv_stride_rows;
+    kv.fp8 = k_scale != nullptr; kv.k_scale = k_scale; kv.v_scale = v_scale;
+    return kv;
+}
+int kv_tmap(CUtensorMap* tm, const KvLayout& kv) {
+    if (kv.fp8) return make_tmap_u8_2d(tm, kv.base, (uint64_t)kv.layer_stride_rows * kv.head_dim / 128, 128, (uint32_t)(kv.head_dim / 2), 128);
+    return make_tmap_bf16_2d(tm, kv.base, (uint64_t)kv.layer_stride_rows, (uint64_t)kv.head_dim, (uint64_t)kv.head_dim, 64, 64);
+}
+
+int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                    const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s);
 }  // namespace
 
 // test-only: materialise the deterministic fixed-order sum of stream-K partials as fp32 [M,N]
@@ -91,11 +106,35 @@ int oa_k_gemm(const void* A, const void* B, int32_t M, int32_t N, int32_t K, int
 int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
                          int32_t max_pages_per_seq, const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs,
                          int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t force_splits, void* stream) {
+    return paged_attention(q, out, one_layer_kv(kv_cache, num_pages, n_kv, head_dim, nullptr, nullptr), block_tables, max_pages_per_seq, ctx_lens,
+                           q_lens, n_seqs, n_heads, force_splits, (cudaStream_t)stream);
+}
+
+int oa_k_paged_attention_fp8(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
+                             int32_t max_pages_per_seq, const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs,
+                             int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t force_splits, float k_scale, float v_scale, void* stream) {
+    return paged_attention(q, out, one_layer_kv(kv_cache, num_pages, n_kv, head_dim, &k_scale, &v_scale), block_tables, max_pages_per_seq, ctx_lens,
+                           q_lens, n_seqs, n_heads, force_splits, (cudaStream_t)stream);
+}
+
+int oa_k_kv_write_fp8(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos, const float* rope_sin, void* q_out,
+                      void* kv_cache, int32_t num_pages, int32_t T, int32_t n_heads, int32_t n_kv, int32_t head_dim, float k_scale, float v_scale,
+                      void* stream) {
     cudaStream_t s = (cudaStream_t)stream;
-    KvLayout kv{}; kv.base = const_cast<void*>(kv_cache); kv.page_size = 64; kv.n_kv = n_kv; kv.head_dim = head_dim; kv.num_pages = num_pages;
-    kv.kv_stride_rows = (int64_t)num_pages * n_kv * 64; kv.layer_stride_rows = 2 * kv.kv_stride_rows;
+    const KvLayout kv = one_layer_kv(kv_cache, num_pages, n_kv, head_dim, &k_scale, &v_scale);
+    cudaError_t e = launch_rope_kv_write(qkv, positions, slots, rope_cos, rope_sin, q_out, kv, 0, T, n_heads, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_of(e);
+}
+
+}  // extern "C"
+
+namespace {
+int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                    const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s) {
+    const int n_kv = kv.n_kv, head_dim = kv.head_dim;
     CUtensorMap tm;
-    if (make_tmap_bf16_2d(&tm, kv_cache, (uint64_t)kv.layer_stride_rows, (uint64_t)head_dim, (uint64_t)head_dim, 64, 64) != 0) return OA_ERR_INTERNAL;
+    if (kv_tmap(&tm, kv) != 0) return OA_ERR_INTERNAL;
     const float scale_log2e = (1.0f / std::sqrt((float)head_dim)) * 1.4426950408889634f;
     const int grp = n_heads / n_kv;
     bool decode = true; int total_q = 0;
@@ -138,6 +177,9 @@ int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     return rc_of(e);
 }
+}  // namespace
+
+extern "C" {
 
 
 int oa_host_apply_chat_template(const char* config_json, const oa_msg* msgs, int32_t n_msgs, int32_t* out_ids, int32_t cap, int32_t* n_out) {
@@ -230,9 +272,10 @@ int oa_host_model_info(const char* config_json, char* buf, size_t n) {
         ModelConfig c; EngineOptions eo; parse_config(config_json ? config_json : "{}", c, eo);
         std::snprintf(buf, n, "{\"model\": \"%s\", \"hidden\": %d, \"n_layers\": %d, \"n_heads\": %d, \"n_kv_heads\": %d, \"head_dim\": %d, "
                       "\"ffn\": %d, \"vocab\": %d, \"tie_embeddings\": %d, \"qkv_bias\": %d, \"rope_scaling\": %d, \"rope_theta\": %.1f, "
-                      "\"rms_eps\": %g, \"template\": \"%s\", \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu}",
+                      "\"rms_eps\": %g, \"template\": \"%s\", \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu%s}",
                       c.name.c_str(), c.hidden, c.n_layers, c.n_heads, c.n_kv_heads, c.head_dim, c.ffn, c.vocab, c.tie_embeddings, c.qkv_bias,
-                      c.rope_scaling, c.rope_theta, c.rms_eps, c.chat_template.c_str(), c.decode_weight_bytes(), c.kv_bytes_per_token());
+                      c.rope_scaling, c.rope_theta, c.rms_eps, c.chat_template.c_str(), c.decode_weight_bytes(), c.kv_bytes_per_token(),
+                      c.kv_fp8() ? ", \"kv_cache_dtype\": \"fp8_e4m3\"" : "");
     } catch (const std::exception&) { return OA_ERR_BAD_REQUEST; }
     return OA_OK;
 }

@@ -95,6 +95,26 @@ OA_DEVINL uint4 rms_scale_bf16x8(uint4 v, float r, uint4 g) {
 OA_DEVINL uint16_t* kv_row(uint16_t* kv_base, int64_t plane_row0, int page, int nkv, int head, int page_size, int off, int D) {
     return kv_base + (size_t)(plane_row0 + ((int64_t)page * nkv + head) * page_size + off) * D;
 }
+// fp8 KV cache (e4m3, OCP "fn" variant).  Four fp32 -> four bytes (byte i = lane i), round to nearest even, saturating to +-448: the
+// NaN codes 0x7f / 0xff are never written.  cvt.*x2 takes the high operand first.
+OA_DEVINL uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+    uint16_t lo, hi;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
+    return (uint32_t)lo | ((uint32_t)hi << 16);
+}
+// 8 fp32 times `mul` -> 8 e4m3 bytes
+OA_DEVINL uint2 pack_e4m3x8(const float* f, float mul) {
+    return make_uint2(pack_e4m3x4(f[0] * mul, f[1] * mul, f[2] * mul, f[3] * mul), pack_e4m3x4(f[4] * mul, f[5] * mul, f[6] * mul, f[7] * mul));
+}
+// two e4m3 bytes (lo = byte 0) -> bf16x2, exact: every e4m3 value is an f16 normal or zero, and every f16 value of that set a bf16 value
+OA_DEVINL uint32_t e4m3x2_to_bf16x2(uint16_t v) {
+    uint32_t h;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(v));
+    float lo, hi;
+    asm("{\n\t.reg .f16 l, u;\n\tmov.b32 {l, u}, %2;\n\tcvt.f32.f16 %0, l;\n\tcvt.f32.f16 %1, u;\n\t}" : "=f"(lo), "=f"(hi) : "r"(h));
+    return pack_bf16x2(lo, hi);
+}
 
 OA_DEVINL uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // ---------------------------------------------------------------------------------------------
@@ -298,6 +318,20 @@ OA_DEVINL void wgmma_rs_m64n128_tb(float (&d)[64], const uint32_t (&a)[4], uint6
         "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
         "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
         "}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+        : OA_F16(0), OA_F16(16), OA_F16(32), OA_F16(48)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_rs_m64n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
         : OA_F16(0), OA_F16(16), OA_F16(32), OA_F16(48)
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc) : "memory");
 }

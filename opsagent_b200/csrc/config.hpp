@@ -70,7 +70,10 @@ struct ModelConfig {
     int q_dim() const { return n_heads * head_dim; }
     int kv_dim() const { return n_kv_heads * head_dim; }
     int qkv_dim() const { return q_dim() + 2 * kv_dim(); }
-    size_t kv_bytes_per_token() const { return (size_t)2 * n_layers * kv_dim() * 2; }
+    std::string kv_cache_dtype = "bf16";    // paged KV cache storage: "bf16" or "fp8_e4m3" (one byte per element, per-layer K / V scales)
+    bool kv_fp8() const { return kv_cache_dtype == "fp8_e4m3"; }
+    int kv_elem_bytes() const { return kv_fp8() ? 1 : 2; }
+    size_t kv_bytes_per_token() const { return (size_t)2 * n_layers * kv_dim() * kv_elem_bytes(); }
     double decode_weight_bytes() const {   // W_dec of SURVEY.md §8d: all layers + final norm + lm_head
         double per = (double)qkv_dim() * hidden + (double)hidden * q_dim() + 3.0 * ffn * hidden + 2.0 * hidden + (qkv_bias ? qkv_dim() : 0);
         return 2.0 * (per * n_layers + hidden + (double)vocab * hidden);
@@ -140,6 +143,7 @@ inline void parse_config(const std::string& json, ModelConfig& m, EngineOptions&
     F("init_std", m.init_std);
     m.seed = (uint64_t)j.i("seed", (int64_t)m.seed);
     m.chat_template = j.s("template", m.chat_template);
+    m.kv_cache_dtype = j.s("kv_cache_dtype", m.kv_cache_dtype);
     I("device", o.device); o.kv_gb = j.f("kv_gb", o.kv_gb); I("num_pages", o.num_pages); I("max_batch", o.max_batch);
     I("max_seq_len", o.max_seq_len); I("max_step_tokens", o.max_step_tokens); I("max_queue", o.max_queue);
     I("bn_qkv", o.bn_qkv); I("bn_o", o.bn_o); I("bn_gu", o.bn_gu); I("bn_down", o.bn_down); I("bn_lm", o.bn_lm);
@@ -150,6 +154,7 @@ inline void parse_config(const std::string& json, ModelConfig& m, EngineOptions&
     if (m.n_heads % m.n_kv_heads != 0 || m.n_heads / m.n_kv_heads > 8) throw std::runtime_error("GQA group must divide n_heads and be <= 8");
     if (m.hidden % 64 || m.ffn % 64 || m.vocab % 8) throw std::runtime_error("hidden/ffn must be multiples of 64, vocab of 8");
     if (m.chat_template != "llama3" && m.chat_template != "chatml") throw std::runtime_error("template must be llama3 or chatml");
+    if (m.kv_cache_dtype != "bf16" && m.kv_cache_dtype != "fp8_e4m3") throw std::runtime_error("kv_cache_dtype must be bf16 or fp8_e4m3");
     if (o.max_seq_len % 64) o.max_seq_len = (o.max_seq_len + 63) / 64 * 64;
     if (o.tp < 1 || o.tp > 8 || o.tp_rank < 0 || o.tp_rank >= o.tp) throw std::runtime_error("tp must be 1..8 and 0 <= tp_rank < tp");
     if (o.tp > 1 && (m.n_kv_heads % o.tp || m.n_heads % o.tp || (m.ffn / o.tp) % 64 || m.ffn % o.tp || (m.vocab / o.tp) % 8 || m.vocab % o.tp))

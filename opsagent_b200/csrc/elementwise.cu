@@ -94,15 +94,13 @@ __global__ void rope_kv_write_kernel(const uint16_t* __restrict__ qkv, const SkR
         float av[8], bv[8];
         unpack_bf16x8(*reinterpret_cast<const uint4*>(src + i0), av);
         unpack_bf16x8(*reinterpret_cast<const uint4*>(src + i0 + half), bv);
-        uint16_t* dst = rope_dst_row(a, t, head, page, off);
-        rope_bf16x8(av, bv, cr + i0, sr + i0, *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
+        rope_store8(a, t, head, page, off, i0, av, bv, cr + i0, sr + i0);
     }
     // V: straight copy into the V plane
     const int n_v = a.nkv * (D >> 3);
     for (int w = threadIdx.x; w < n_v; w += blockDim.x) {
         const int head = w / (D >> 3), i0 = (w - head * (D >> 3)) * 8;
-        *reinterpret_cast<uint4*>(rope_dst_row(a, t, a.nh + a.nkv + head, page, off) + i0) =
-            *reinterpret_cast<const uint4*>(row + (size_t)(a.nh + a.nkv + head) * D + i0);
+        kv_store8(a, t, a.nh + a.nkv + head, page, off, i0, *reinterpret_cast<const uint4*>(row + (size_t)(a.nh + a.nkv + head) * D + i0));
     }
 }
 cudaError_t launch_rope_kv_write(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos,
@@ -171,6 +169,8 @@ SkRopeArgs make_sk_rope_args(const void* bias, const int32_t* positions, const i
     a.q_out = reinterpret_cast<uint16_t*>(q_out); a.kv_base = reinterpret_cast<uint16_t*>(kv.base);
     a.k_plane_row0 = (int64_t)layer * kv.layer_stride_rows; a.v_plane_row0 = a.k_plane_row0 + kv.kv_stride_rows;
     a.page_size = kv.page_size; a.nh = nh; a.nkv = kv.n_kv; a.D = kv.head_dim;
+    a.kv_fp8 = kv.fp8;
+    if (kv.fp8) { a.k_inv_scale = 1.0f / kv.k_scale[layer]; a.v_inv_scale = 1.0f / kv.v_scale[layer]; }
     return a;
 }
 cudaError_t launch_sk_rope_kv_write(const StreamK& sk, const void* bias, const int32_t* positions, const int32_t* slots,

@@ -130,14 +130,12 @@ __global__ void OA_GEMM_REGS gemm_clusterk_kernel(const __grid_constant__ CUtens
                 const int slot_tok = a.slots[row], page = slot_tok / a.page_size, off = slot_tok - page * a.page_size;
                 qkv_finish8(a.bias, col_lo, acc[0]);
                 qkv_finish8(a.bias, col_hi, acc[1]);
-                uint16_t* dst = rope_dst_row(a, row, head, page, off);
                 if (head >= a.nh + a.nkv) {                       // V: straight copy of both halves into the V plane
-                    *reinterpret_cast<uint4*>(dst + i0) = pack_bf16x8(acc[0]);
-                    *reinterpret_cast<uint4*>(dst + i0 + half) = pack_bf16x8(acc[1]);
+                    kv_store8(a, row, head, page, off, i0, pack_bf16x8(acc[0]));
+                    kv_store8(a, row, head, page, off, i0 + half, pack_bf16x8(acc[1]));
                 } else {
                     const int pos = a.positions[row];
-                    rope_bf16x8(acc[0], acc[1], a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0,
-                                *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
+                    rope_store8(a, row, head, page, off, i0, acc[0], acc[1], a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0);
                 }
             }
         }

@@ -459,9 +459,8 @@ __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtenso
 #pragma unroll
                                     for (int h = 0; h < 4; ++h) qkv_finish8(a.bias, col0 + 8 * h, vv + 8 * h);
                                     if (live) {
-                                        uint4* dst = reinterpret_cast<uint4*>(rope_dst_row(a, row, head, page, off) + i0);
 #pragma unroll
-                                        for (int h = 0; h < 4; ++h) dst[h] = pack_bf16x8(vv + 8 * h);
+                                        for (int h = 0; h < 4; ++h) kv_store8(a, row, head, page, off, i0 + 8 * h, pack_bf16x8(vv + 8 * h));
                                     }
                                     continue;
                                 }
@@ -477,9 +476,8 @@ __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtenso
                                 if (live) {
                                     const float* cr = a.rope_cos + (size_t)pos * half + i0;
                                     const float* sr = a.rope_sin + (size_t)pos * half + i0;
-                                    uint4* dst = reinterpret_cast<uint4*>(rope_dst_row(a, row, head, page, off) + i0);
 #pragma unroll
-                                    for (int h = 0; h < 4; ++h) rope_bf16x8(av + 8 * h, bv + 8 * h, cr + 8 * h, sr + 8 * h, dst[h], dst[h + half / 8]);
+                                    for (int h = 0; h < 4; ++h) rope_store8(a, row, head, page, off, i0 + 8 * h, av + 8 * h, bv + 8 * h, cr + 8 * h, sr + 8 * h);
                                 }
                             }
                         }

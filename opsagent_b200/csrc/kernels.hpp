@@ -13,6 +13,8 @@ namespace oa {
 // 128-byte swizzle.  Returns 0 on success (driver entry point resolved through the runtime, no -lcuda).
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
                       uint32_t box_rows, uint32_t box_cols);
+// 2D row-major byte tensor [rows, cols] (dense rows), box = {box_cols(<=128), box_rows(<=256)}, 128-byte swizzle (the fp8 KV pool)
+int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols);
 
 // ---- GEMM (gemm_wgmma.cu): C[M,N] = A[M,K] . B[N,K]^T, bf16 in, fp32 accumulate in registers ----
 enum GemmEpilogue : int {
@@ -71,6 +73,7 @@ cudaError_t launch_sk_swiglu(const StreamK& sk, void* act, int T, int F, cudaStr
 struct SkRopeArgs {       // q/k/v from the qkv projection's partials (+ bias): sum -> bf16 -> RoPE -> bf16 (the oracle's order)
     const uint16_t* bias; const int32_t* positions; const int32_t* slots; const float* rope_cos; const float* rope_sin;
     uint16_t* q_out; uint16_t* kv_base; int64_t k_plane_row0, v_plane_row0; int32_t page_size, nh, nkv, D;
+    int32_t kv_fp8; float k_inv_scale, v_inv_scale;   // fp8 cache: stored byte = e4m3(value * inv_scale) (KvLayout)
 };
 // o / down projection with the residual add finished inside the GEMM: x[M, ldx] (bf16, in place) += A.B^T, bit-identical to
 // launch_gemm_streamk + the sum/residual half of launch_sk_resid_rmsnorm.  Follow with launch_rmsnorm_wide for the norm.
@@ -102,10 +105,14 @@ cudaError_t launch_gather_rows(const void* x, const int32_t* rows, void* out, in
 // RoPE (HF rotate_half pairing) on q and k in `qkv` [T, (nh+2nkv)*D]; rotated q -> q_out [T, nh*D];
 // rotated k and v -> paged KV cache rows.  slot[t] = page*page_size + offset of token t.
 struct KvLayout {
-    void* base;            // bf16 rows of D elements
+    void* base;            // rows of D elements (bf16, or e4m3 bytes when fp8)
     int64_t layer_stride_rows;   // rows between consecutive layers (= 2 * num_pages * nkv * page_size)
     int64_t kv_stride_rows;      // rows between K and V planes of a layer (= num_pages * nkv * page_size)
     int32_t page_size, n_kv, head_dim, num_pages;
+    // fp8 (e4m3) cache: one (page, kv head) block is 64 * D bytes; K as [64 tokens][D], V transposed as [D][64 tokens].  The byte x of
+    // layer l decodes to e4m3(x) * k_scale[l] (K) or * v_scale[l] (V); k_scale / v_scale are host arrays of the layers' scales
+    int32_t fp8;
+    const float* k_scale; const float* v_scale;
 };
 // same, but q/k/v come from stream-K partials (+ bias): sum -> bf16 round -> RoPE -> bf16 round (the oracle's order)
 cudaError_t launch_sk_rope_kv_write(const StreamK& sk, const void* bias, const int32_t* positions, const int32_t* slots,
@@ -139,7 +146,7 @@ struct DecodeAttnParams {
     float* part_o; float* part_ml; // partial workspace: [slots, group, D] fp32 and [slots, group, 2]
     int32_t* merge_counters;       // [items], zero at the start of a step; the CTA that completes an item's last piece merges it (null: separate merge kernel)
     int32_t layer, n_heads, n_kv;
-    float scale_log2e;             // (1/sqrt(D)) * log2(e)
+    float scale_log2e;             // (1/sqrt(D)) * log2(e)  (the fp8 launcher multiplies in the layer's k_scale)
 };
 cudaError_t launch_decode_attention(const CUtensorMap* tm_kv, const KvLayout& kv, const DecodeAttnParams& p, cudaStream_t s);
 struct MergeItem { int32_t seq, kvh, slot_begin, n_slots; };

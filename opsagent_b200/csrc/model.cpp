@@ -118,6 +118,7 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
         }
     }
 
+    kv_k_scale.assign(L, 1.0f); kv_v_scale.assign(L, 1.0f);
     if (!opt.weights.empty()) load_checkpoint(opt.weights);
 
     // ---- RoPE table ----
@@ -162,7 +163,7 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     cuda_check(cudaMallocHost(&h_out_ids, (size_t)MS * 4), "cudaMallocHost");
 
     // ---- paged KV pool ----
-    const size_t page_bytes = (size_t)2 * L * nkv_l * 64 * D * 2;    // all layers, K and V, of 64 tokens (this rank's kv heads)
+    const size_t page_bytes = (size_t)2 * L * nkv_l * 64 * D * cfg.kv_elem_bytes();    // all layers, K and V, of 64 tokens (this rank's kv heads)
     if (opt.num_pages > 0) num_pages = opt.num_pages;
     else {
         size_t free_b = 0, total_b = 0;
@@ -177,11 +178,14 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     if ((double)plane_rows * 2 * L >= 2147483647.0) { num_pages = (int)(2147483647.0 / (2.0 * L * nkv_l * 64)) - 1; }
     kv.page_size = 64; kv.n_kv = nkv_l; kv.head_dim = D; kv.num_pages = num_pages;
     kv.kv_stride_rows = (int64_t)num_pages * nkv_l * 64; kv.layer_stride_rows = 2 * kv.kv_stride_rows;
+    kv.fp8 = cfg.kv_fp8(); kv.k_scale = kv_k_scale.data(); kv.v_scale = kv_v_scale.data();
     kv_pool_bytes = (size_t)num_pages * page_bytes;
     kv.base = dmalloc(kv_pool_bytes);
-    cuda_check(cudaMemsetAsync(kv.base, 0, kv_pool_bytes, stream), "kv memset");   // stale pages must hold finite values (0*NaN)
+    cuda_check(cudaMemsetAsync(kv.base, 0, kv_pool_bytes, stream), "kv memset");   // stale pages must hold finite values (0*NaN; e4m3 0x00 = +0)
     {
-        int r = make_tmap_bf16_2d(&tm_kv, kv.base, (uint64_t)kv.layer_stride_rows * L, (uint64_t)D, (uint64_t)D, 64, 64);
+        // fp8: the pool as rows of 128 bytes, one (page, kv head) block of K or V per box
+        int r = kv.fp8 ? make_tmap_u8_2d(&tm_kv, kv.base, (uint64_t)(kv_pool_bytes / 128), 128, (uint32_t)(D / 2), 128)
+                       : make_tmap_bf16_2d(&tm_kv, kv.base, (uint64_t)kv.layer_stride_rows * L, (uint64_t)D, (uint64_t)D, 64, 64);
         if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for the KV pool (code " + std::to_string(r) + ")");
     }
 
@@ -225,21 +229,51 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
 }
 
 // ---- Hugging Face checkpoint loading (Llama / Qwen2 naming) --------------------------------------------------------
+static float f16_bits_to_f32(uint16_t hb) {
+    const uint32_t h = hb, sign = (h & 0x8000u) << 16, e = (h >> 10) & 31, m = h & 1023; uint32_t f;
+    if (e == 0) { if (m == 0) f = sign; else { int sh = 0; uint32_t mm = m; while (!(mm & 1024)) { mm <<= 1; ++sh; } f = sign | ((uint32_t)(113 - sh) << 23) | ((mm & 1023) << 13); } }
+    else if (e == 31) f = sign | 0x7f800000u | (m << 13);
+    else f = sign | ((e + 112) << 23) | (m << 13);
+    float x; std::memcpy(&x, &f, 4); return x;
+}
 static void to_bf16_rows(const StTensor& t, int64_t C, int64_t row, int64_t col0, int64_t cols, uint16_t* dst) {
     if (t.dtype == "BF16") { std::memcpy(dst, reinterpret_cast<const uint16_t*>(t.data) + row * C + col0, (size_t)cols * 2); return; }
     if (t.dtype == "F32") { const float* s = reinterpret_cast<const float*>(t.data) + row * C + col0; for (int64_t i = 0; i < cols; ++i) dst[i] = f32_to_bf16_bits(s[i]); return; }
     if (t.dtype == "F16") {
         const uint16_t* s = reinterpret_cast<const uint16_t*>(t.data) + row * C + col0;
-        for (int64_t i = 0; i < cols; ++i) {
-            const uint32_t h = s[i], sign = (h & 0x8000u) << 16, e = (h >> 10) & 31, m = h & 1023; uint32_t f;
-            if (e == 0) { if (m == 0) f = sign; else { int sh = 0; uint32_t mm = m; while (!(mm & 1024)) { mm <<= 1; ++sh; } f = sign | ((uint32_t)(113 - sh) << 23) | ((mm & 1023) << 13); } }
-            else if (e == 31) f = sign | 0x7f800000u | (m << 13);
-            else f = sign | ((e + 112) << 23) | (m << 13);
-            float x; std::memcpy(&x, &f, 4); dst[i] = f32_to_bf16_bits(x);
-        }
+        for (int64_t i = 0; i < cols; ++i) dst[i] = f32_to_bf16_bits(f16_bits_to_f32(s[i]));
         return;
     }
     throw std::runtime_error("unsupported checkpoint dtype " + t.dtype);
+}
+
+// fp8 KV cache scales (compressed-tensors / vLLM naming): model.layers.{l}.self_attn.k_scale / v_scale, shape [] or [1], F32 / BF16 / F16,
+// finite and > 0, present for every layer or for none (then 1.0)
+static void load_kv_scales(const SafeTensors& st, int L, std::vector<float>& ks, std::vector<float>& vs) {
+    auto scalar = [&](const std::string& name) -> float {
+        const StTensor& t = st.get(name);
+        if (!(t.shape.empty() || (t.shape.size() == 1 && t.shape[0] == 1))) throw std::runtime_error("checkpoint tensor " + name + " must have shape [] or [1]");
+        float v;
+        if (t.dtype == "F32") std::memcpy(&v, t.data, 4);
+        else if (t.dtype == "BF16") { uint16_t b; std::memcpy(&b, t.data, 2); const uint32_t u = (uint32_t)b << 16; std::memcpy(&v, &u, 4); }
+        else if (t.dtype == "F16") { uint16_t b; std::memcpy(&b, t.data, 2); v = f16_bits_to_f32(b); }
+        else throw std::runtime_error("checkpoint tensor " + name + " has unsupported dtype " + t.dtype);
+        if (!std::isfinite(v) || v <= 0.f) throw std::runtime_error("checkpoint tensor " + name + " must be finite and > 0");
+        return v;
+    };
+    int nk = 0, nv = 0;
+    for (int l = 0; l < L; ++l) {
+        const std::string p = "model.layers." + std::to_string(l) + ".self_attn.";
+        nk += st.has(p + "k_scale"); nv += st.has(p + "v_scale");
+    }
+    if (nk == 0 && nv == 0) return;
+    for (const auto& c : {std::make_pair("k_scale", nk), std::make_pair("v_scale", nv)})
+        if (c.second != L) throw std::runtime_error("checkpoint has self_attn." + std::string(c.first) + " for " + std::to_string(c.second) + " of " +
+                                                    std::to_string(L) + " layers: KV cache scales must be given for every layer or for none");
+    for (int l = 0; l < L; ++l) {
+        const std::string p = "model.layers." + std::to_string(l) + ".self_attn.";
+        ks[l] = scalar(p + "k_scale"); vs[l] = scalar(p + "v_scale");
+    }
 }
 
 void DeviceModel::load_checkpoint(const std::string& path) {
@@ -268,6 +302,7 @@ void DeviceModel::load_checkpoint(const std::string& path) {
         for (int64_t i = 0; i < rows; ++i) to_bf16_rows(t, C, row0 + i, col0, cols, buf.data() + (size_t)i * cols);
         cuda_check(cudaMemcpy(dst, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
     };
+    if (cfg.kv_fp8()) load_kv_scales(st, L, kv_k_scale, kv_v_scale);
     slice("model.embed_tokens.weight", V, H, 0, V, 0, H, embed);
     slice("model.norm.weight", 1, H, 0, 1, 0, H, final_norm);
     if (!cfg.tie_embeddings) slice(st.has("lm_head.weight") ? "lm_head.weight" : "model.embed_tokens.weight", V, H, r * V_l, V_l, 0, H, lm_head.ptr);

@@ -62,6 +62,7 @@ public:
     int mask_words = 0, mask_slots = 0, max_mask_updates = 0;    // token-mask table geometry (words = ceil(vocab / 32))
     size_t weight_bytes = 0, kv_pool_bytes = 0;
     KvLayout kv{}; CUtensorMap tm_kv;
+    std::vector<float> kv_k_scale, kv_v_scale;      // per layer (fp8 cache: from the checkpoint, else 1.0)
     // instrumentation
     bool profile_attn = false; double attn_ms_accum = 0; std::vector<cudaEvent_t> ev;
     // in-situ per-kernel timing (events after every launch, warm caches, real launch gaps): OA_PROFILE_ALL=1

@@ -1,7 +1,7 @@
 // sk_consumers.cuh — the consumers of stream-K partials as device functions: each adds a tile's fp32 partials in CTA
 // order (deterministic) and finishes the op with the bf16x8 epilogue helpers of common.cuh.  The stand-alone consumer kernels
 // (elementwise.cu, tp_comm.cu) run these functions; the GEMM epilogues that finish an op themselves (gemm_wgmma.cu FUSE=1/2/3,
-// gemm_clusterk.cu) sum in the same order and call the same helpers and rope_dst_row, so every path produces bit-identical results.
+// gemm_clusterk.cu) sum in the same order and call the same helpers and kv_store8, so every path produces bit-identical results.
 #pragma once
 #include "common.cuh"
 #include "kernels.hpp"
@@ -140,6 +140,32 @@ OA_DEVINL uint16_t* rope_dst_row(const SkRopeArgs& a, int t, int head, int page,
     return kv_row(a.kv_base, a.v_plane_row0, page, a.nkv, head - a.nh - a.nkv, a.page_size, off, a.D);
 }
 
+// Stores 8 finished bf16 lanes (columns i0..i0+7 of head `head`) where rope_dst_row points: q_out, or the paged K / V plane.  Every
+// writer of the KV cache stores through here.  fp8 cache: byte = e4m3(bf16 value * inv_scale); K as [token][D] (8 consecutive bytes), V
+// transposed inside its (page, kv head) block as [D][page_size] (8 bytes page_size apart).
+OA_DEVINL void kv_store8(const SkRopeArgs& a, int t, int head, int page, int off, int i0, uint4 v) {
+    if (!a.kv_fp8 || head < a.nh) { *reinterpret_cast<uint4*>(rope_dst_row(a, t, head, page, off) + i0) = v; return; }
+    float f[8];
+    unpack_bf16x8(v, f);
+    uint8_t* base = reinterpret_cast<uint8_t*>(a.kv_base);
+    if (head < a.nh + a.nkv) {
+        *reinterpret_cast<uint2*>(base + (size_t)(a.k_plane_row0 + ((int64_t)page * a.nkv + head - a.nh) * a.page_size + off) * a.D + i0) =
+            pack_e4m3x8(f, a.k_inv_scale);
+        return;
+    }
+    const uint2 b = pack_e4m3x8(f, a.v_inv_scale);
+    uint8_t* col = base + (size_t)(a.v_plane_row0 + ((int64_t)page * a.nkv + head - a.nh - a.nkv) * a.page_size) * a.D + (size_t)i0 * a.page_size + off;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) col[(size_t)k * a.page_size] = (uint8_t)(((k < 4 ? b.x : b.y) >> (8 * (k & 3))) & 0xff);
+}
+// RoPE of 8 (lo, hi) pairs of head `head` (columns i0.. and i0 + D/2..) and the store of both halves
+OA_DEVINL void rope_store8(const SkRopeArgs& a, int t, int head, int page, int off, int i0, const float* lo, const float* hi, const float* cs, const float* sn) {
+    uint4 ra, rb;
+    rope_bf16x8(lo, hi, cs, sn, ra, rb);
+    kv_store8(a, t, head, page, off, i0, ra);
+    kv_store8(a, t, head, page, off, i0 + (a.D >> 1), rb);
+}
+
 OA_DEVINL int sk_rope_items_per_row(const SkRopeArgs& a) { return (a.nh + a.nkv) * (a.D >> 4) + a.nkv * (a.D >> 3); }
 // item w of token row t: w < (nh+nkv)*D/16 rotates 8 (lo, hi) pairs of one q or k head; the rest copy 8 elements of v
 OA_DEVINL void sk_rope_item(const StreamK& sk, const SkRopeArgs& a, int t, int w) {
@@ -154,16 +180,14 @@ OA_DEVINL void sk_rope_item(const StreamK& sk, const SkRopeArgs& a, int t, int w
         sk_sum8_pair(sk, t, head * D + i0, head * D + i0 + half, av, bv);
         qkv_finish8(a.bias, head * D + i0, av);
         qkv_finish8(a.bias, head * D + i0 + half, bv);
-        uint16_t* dst = rope_dst_row(a, t, head, page, off);
-        rope_bf16x8(av, bv, a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0,
-                    *reinterpret_cast<uint4*>(dst + i0), *reinterpret_cast<uint4*>(dst + i0 + half));
+        rope_store8(a, t, head, page, off, i0, av, bv, a.rope_cos + (size_t)pos * half + i0, a.rope_sin + (size_t)pos * half + i0);
     } else {
         const int wv = w - n_rot;
         const int head = a.nh + a.nkv + wv / (D >> 3), i0 = (wv % (D >> 3)) * 8;
         float vv[8];
         sk_sum8(sk, t, head * D + i0, vv);
         qkv_finish8(a.bias, head * D + i0, vv);
-        *reinterpret_cast<uint4*>(rope_dst_row(a, t, head, page, off) + i0) = pack_bf16x8(vv);
+        kv_store8(a, t, head, page, off, i0, pack_bf16x8(vv));
     }
 }
 

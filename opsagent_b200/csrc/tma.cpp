@@ -40,6 +40,20 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
+int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols) {
+    EncodeTiledFn enc = resolve_encode();
+    if (!enc) return -1;
+    if (box_cols > 128 || box_rows > 256 || cols % 16 != 0 || (reinterpret_cast<uintptr_t>(base) & 15)) return -2;
+    cuuint64_t gdim[2] = {cols, rows};
+    cuuint64_t gstride[1] = {cols};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
 static std::atomic<uint64_t> g_launches{0};
 uint64_t launches_total() { return g_launches.load(); }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
