@@ -74,7 +74,7 @@ typedef struct {
 
 /* config_json: {"model":"llama-3-8b"|"llama-3.2-1b"|"qwen2.5-32b"|"llama-3-70b"|custom dims..., "seed":1234,
  *  "device":0, "kv_gb":100, "max_batch":128, "max_seq_len":4096, "max_step_tokens":8192,
- *  "kv_cache_dtype":"bf16"|"fp8_e4m3", ...} — see DESIGN.md */
+ *  "kv_cache_dtype":"bf16"|"fp8_e4m3", "weight_dtype":"bf16"|"fp8_e4m3", ...} — see DESIGN.md */
 OA_API int oa_engine_create(const char* config_json, oa_engine** out);
 OA_API void oa_engine_destroy(oa_engine*);
 /* tensor-parallel groups (config "tp": t, "tp_rank": r, "tp_shm": name; one process per GPU): rank 0 is the engine callers talk
@@ -156,6 +156,17 @@ OA_API int oa_k_paged_attention_fp8(const void* q, void* out, const void* kv_cac
 OA_API int oa_k_kv_write_fp8(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos, const float* rope_sin,
                       void* q_out, void* kv_cache, int32_t num_pages, int32_t T, int32_t n_heads, int32_t n_kv, int32_t head_dim,
                       float k_scale, float v_scale, void* stream);
+/* fp8 (e4m3) projections (weight_dtype "fp8_e4m3").  Row quantiser: bf16 x [R, C] -> e4m3 bytes q [R, C] + fp32 scale [R], per row
+ * s = the smallest power of two with max|x| <= 448 s (all-zero row: 1), q = e4m3(x / s) (C % 16 == 0). */
+OA_API int oa_k_quant_rows_e4m3(const void* x, void* q, float* scale, int32_t R, int32_t C, void* stream);
+/* out = sa[m] * sb[n] * sum_k A[m,k] B[n,k] for e4m3 A [M, K], B [N, K] with fp32 row scales (device pointers); epilogues as oa_k_gemm
+ * (0 store (+ bias), 1 residual, 2 SwiGLU), block_n in {32, 64, 128}; large shapes take the persistent kernel as in oa_k_gemm */
+OA_API int oa_k_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t epilogue,
+                         int32_t block_n, void* out, const void* bias, const void* resid, void* stream);
+/* the same product on the stream-K decode GEMM (M <= 128, block_n 64 / 128): fuse 0 = fp32 out_f32 [M, N] (sum of the partials),
+ * fuse 2 = x [M, N] bf16 += product, finished inside the GEMM */
+OA_API int oa_k_gemm_streamk_fp8(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t block_n,
+                                 int32_t n_ctas, int32_t fuse, void* x, float* out_f32, void* stream);
 /* ---- host-only logic, callable without a GPU (CPU tests) ---- */
 /* chat template + tokenizer of the model described by config_json */
 OA_API int oa_host_apply_chat_template(const char* config_json, const oa_msg* msgs, int32_t n_msgs, int32_t* out_ids, int32_t cap, int32_t* n_out);

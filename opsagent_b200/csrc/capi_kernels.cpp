@@ -19,6 +19,7 @@
 #include "tokenizer.hpp"
 
 using namespace oa;
+namespace oa { int fail_host(int code, const std::string& msg); }      // oa_last_error() message (engine.cpp)
 
 namespace {
 struct DevBuf {
@@ -69,6 +70,46 @@ int oa_k_gemm_streamk(const void* A, const void* B, int32_t M, int32_t N, int32_
     StreamK sk = make_streamk((float*)ws.p, N, K, block_n, n_ctas, M);
     cudaError_t e = launch_gemm_streamk(&tmA, &tmB, M, N, K, sk, s);
     if (e == cudaSuccess) { sk_reduce_f32_kernel<<<M, 256, 0, s>>>(sk, out_f32, M, N); e = cudaGetLastError(); }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_of(e);
+}
+
+int oa_k_quant_rows_e4m3(const void* x, void* q, float* scale, int32_t R, int32_t C, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    cudaError_t e = launch_quant_rows_e4m3(x, (uint8_t*)q, scale, R, C, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_of(e);
+}
+
+// fp8 GEMMs: A [M, K] and B [N, K] e4m3 bytes with fp32 row scales sa [M], sb [N] (device pointers)
+int oa_k_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n,
+                  void* out, const void* bias, const void* resid, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    CUtensorMap tmA, tmB;
+    if (make_tmap_u8_2d(&tmA, A, (uint64_t)M, (uint64_t)K, 128, 128) != 0) return OA_ERR_INTERNAL;
+    if (make_tmap_u8_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint32_t)block_n, 128) != 0) return OA_ERR_INTERNAL;
+    GemmParams p{}; p.M = M; p.N = N; p.K = K; p.out = out; p.ldo = epilogue == EPI_SWIGLU ? N / 2 : N;
+    p.bias = bias; p.resid = resid; p.ldr = N; p.w8 = W8Scales{sa, sb};
+    cudaError_t e = launch_gemm(&tmA, &tmB, p, epilogue, block_n, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_of(e);
+}
+// fused: 0 = plain (fp32 out = the fixed-order sum of the partials), 2 = residual add into x [M, N] bf16 (out_f32 unused)
+int oa_k_gemm_streamk_fp8(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t block_n,
+                          int32_t n_ctas, int32_t fuse, void* x, float* out_f32, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    CUtensorMap tmA, tmB;
+    if (make_tmap_u8_2d(&tmA, A, (uint64_t)M, (uint64_t)K, 128, 128) != 0) return OA_ERR_INTERNAL;
+    if (make_tmap_u8_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint32_t)block_n, 128) != 0) return OA_ERR_INTERNAL;
+    DevBuf ws(streamk_ws_bytes(N, block_n, n_ctas, M)), flags((size_t)SK_MAX_FLAG_TILES * 4);
+    if (!ws.p || !flags.p || cudaMemsetAsync(flags.p, 0, (size_t)SK_MAX_FLAG_TILES * 4, s) != cudaSuccess) return OA_ERR_INTERNAL;
+    StreamK sk = make_streamk((float*)ws.p, N, K, block_n, n_ctas, M, true);
+    cudaError_t e;
+    if (fuse == 2) e = launch_gemm_streamk_resid(&tmA, &tmB, M, N, K, sk, x, N, (unsigned int*)flags.p, s, W8Scales{sa, sb});
+    else if (fuse == 0) {
+        e = launch_gemm_streamk(&tmA, &tmB, M, N, K, sk, s, W8Scales{sa, sb});
+        if (e == cudaSuccess) { sk_reduce_f32_kernel<<<M, 256, 0, s>>>(sk, out_f32, M, N); e = cudaGetLastError(); }
+    } else return OA_ERR_BAD_REQUEST;
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     return rc_of(e);
 }
@@ -272,11 +313,11 @@ int oa_host_model_info(const char* config_json, char* buf, size_t n) {
         ModelConfig c; EngineOptions eo; parse_config(config_json ? config_json : "{}", c, eo);
         std::snprintf(buf, n, "{\"model\": \"%s\", \"hidden\": %d, \"n_layers\": %d, \"n_heads\": %d, \"n_kv_heads\": %d, \"head_dim\": %d, "
                       "\"ffn\": %d, \"vocab\": %d, \"tie_embeddings\": %d, \"qkv_bias\": %d, \"rope_scaling\": %d, \"rope_theta\": %.1f, "
-                      "\"rms_eps\": %g, \"template\": \"%s\", \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu%s}",
+                      "\"rms_eps\": %g, \"template\": \"%s\", \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu%s%s}",
                       c.name.c_str(), c.hidden, c.n_layers, c.n_heads, c.n_kv_heads, c.head_dim, c.ffn, c.vocab, c.tie_embeddings, c.qkv_bias,
                       c.rope_scaling, c.rope_theta, c.rms_eps, c.chat_template.c_str(), c.decode_weight_bytes(), c.kv_bytes_per_token(),
-                      c.kv_fp8() ? ", \"kv_cache_dtype\": \"fp8_e4m3\"" : "");
-    } catch (const std::exception&) { return OA_ERR_BAD_REQUEST; }
+                      c.kv_fp8() ? ", \"kv_cache_dtype\": \"fp8_e4m3\"" : "", c.w_fp8() ? ", \"weight_dtype\": \"fp8_e4m3\"" : "");
+    } catch (const std::exception& e) { return fail_host(OA_ERR_BAD_REQUEST, e.what()); }
     return OA_OK;
 }
 

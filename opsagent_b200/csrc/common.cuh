@@ -341,6 +341,72 @@ OA_DEVINL void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t 
     else if constexpr (N == 64) wgmma_m64n64(d, da, db, acc);
     else { static_assert(N == 128, "wgmma N in {32, 64, 128}"); wgmma_m64n128(d, da, db, acc); }
 }
+// D[64 x N] (+)= A[64 x 32] . B[N x 32]^T with e4m3 operands (both K-major, same descriptors: 32 bytes of K per instruction), fp32 out.
+// The tensor core keeps only about 14 mantissa bits of the running sum across the k32 steps: callers sum a few steps here and promote.
+OA_DEVINL void wgmma_e4m3_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1;\n\t}"
+        : OA_F16(0)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_e4m3_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1;\n\t}"
+        : OA_F16(0), OA_F16(16)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+OA_DEVINL void wgmma_e4m3_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1;\n\t}"
+        : OA_F16(0), OA_F16(16), OA_F16(32), OA_F16(48)
+        : "l"(da), "l"(db), "r"(acc) : "memory");
+}
+template <int N>
+OA_DEVINL void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+    if constexpr (N == 32) wgmma_e4m3_m64n32(d, da, db, acc);
+    else if constexpr (N == 64) wgmma_e4m3_m64n64(d, da, db, acc);
+    else { static_assert(N == 128, "wgmma N in {32, 64, 128}"); wgmma_e4m3_m64n128(d, da, db, acc); }
+}
+// Row scale of the fp8 (e4m3) projections and their inputs: the smallest power of two s with amax <= 448 * s (amax = 0: 1), as a normal
+// fp32.  From the bits of amax = 1.f * 2^(e-127): 448 * 2^(e-135) = 1.75 * 2^(e-127), so s = 2^(e-135) when 1.f <= 1.75, else 2^(e-134).
+__host__ OA_DEVINL float w8_row_scale(float amax) {
+    uint32_t u;
+#ifdef __CUDA_ARCH__
+    u = __float_as_uint(amax);
+#else
+    memcpy(&u, &amax, 4);
+#endif
+    u &= 0x7fffffffu;
+    if (u == 0) return 1.0f;
+    const int e = (int)(u >> 23);
+    int k = e == 0 ? -126 : e - 135 + ((u & 0x7fffffu) > 0x600000u ? 1 : 0);
+    k = k < -126 ? -126 : k;
+    const uint32_t sb = (uint32_t)(k + 127) << 23;
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(sb);
+#else
+    float s; memcpy(&s, &sb, 4); return s;
+#endif
+}
 
 // fp32 accumulator tile [rows][N] in shared memory, 16-byte chunks XOR-swizzled by (row & 7): a warp storing its wgmma fragment
 // and a warp reading 32 consecutive columns of 32 rows (one row per lane) are both free of bank conflicts.  N >= 32.

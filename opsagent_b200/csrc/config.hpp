@@ -74,9 +74,16 @@ struct ModelConfig {
     bool kv_fp8() const { return kv_cache_dtype == "fp8_e4m3"; }
     int kv_elem_bytes() const { return kv_fp8() ? 1 : 2; }
     size_t kv_bytes_per_token() const { return (size_t)2 * n_layers * kv_dim() * kv_elem_bytes(); }
+    // projection weights (qkv, o, gate/up, down): "bf16", or "fp8_e4m3" (one byte per element plus one fp32 scale per output row; W8A8 GEMMs
+    // with per-token activation scales).  Embedding, LM head, norms and biases stay bf16.
+    std::string weight_dtype = "bf16";
+    bool w_fp8() const { return weight_dtype == "fp8_e4m3"; }
     double decode_weight_bytes() const {   // W_dec of SURVEY.md §8d: all layers + final norm + lm_head
-        double per = (double)qkv_dim() * hidden + (double)hidden * q_dim() + 3.0 * ffn * hidden + 2.0 * hidden + (qkv_bias ? qkv_dim() : 0);
-        return 2.0 * (per * n_layers + hidden + (double)vocab * hidden);
+        const double proj = (double)qkv_dim() * hidden + (double)hidden * q_dim() + 3.0 * ffn * hidden;
+        const double rows = (double)qkv_dim() + hidden + 2.0 * ffn + hidden;            // one fp32 scale per output row (fp8)
+        const double other = 2.0 * hidden + (qkv_bias ? qkv_dim() : 0);
+        if (w_fp8()) return (proj + 4.0 * rows + 2.0 * other) * n_layers + 2.0 * (hidden + (double)vocab * hidden);
+        return 2.0 * ((proj + other) * n_layers + hidden + (double)vocab * hidden);
     }
 };
 
@@ -144,6 +151,7 @@ inline void parse_config(const std::string& json, ModelConfig& m, EngineOptions&
     m.seed = (uint64_t)j.i("seed", (int64_t)m.seed);
     m.chat_template = j.s("template", m.chat_template);
     m.kv_cache_dtype = j.s("kv_cache_dtype", m.kv_cache_dtype);
+    m.weight_dtype = j.s("weight_dtype", m.weight_dtype);
     I("device", o.device); o.kv_gb = j.f("kv_gb", o.kv_gb); I("num_pages", o.num_pages); I("max_batch", o.max_batch);
     I("max_seq_len", o.max_seq_len); I("max_step_tokens", o.max_step_tokens); I("max_queue", o.max_queue);
     I("bn_qkv", o.bn_qkv); I("bn_o", o.bn_o); I("bn_gu", o.bn_gu); I("bn_down", o.bn_down); I("bn_lm", o.bn_lm);
@@ -155,6 +163,9 @@ inline void parse_config(const std::string& json, ModelConfig& m, EngineOptions&
     if (m.hidden % 64 || m.ffn % 64 || m.vocab % 8) throw std::runtime_error("hidden/ffn must be multiples of 64, vocab of 8");
     if (m.chat_template != "llama3" && m.chat_template != "chatml") throw std::runtime_error("template must be llama3 or chatml");
     if (m.kv_cache_dtype != "bf16" && m.kv_cache_dtype != "fp8_e4m3") throw std::runtime_error("kv_cache_dtype must be bf16 or fp8_e4m3");
+    if (m.weight_dtype != "bf16" && m.weight_dtype != "fp8_e4m3") throw std::runtime_error("weight_dtype must be bf16 or fp8_e4m3");
+    if (m.w_fp8() && o.tp != 1) throw std::runtime_error("weight_dtype fp8_e4m3 needs tp = 1 (row-parallel shards would need whole-row weight scales)");
+    if (m.w_fp8() && o.sk_clusterk != 0) throw std::runtime_error("weight_dtype fp8_e4m3 needs sk_clusterk = 0 (the cluster split-K GEMM is bf16 only)");
     if (o.max_seq_len % 64) o.max_seq_len = (o.max_seq_len + 63) / 64 * 64;
     if (o.tp < 1 || o.tp > 8 || o.tp_rank < 0 || o.tp_rank >= o.tp) throw std::runtime_error("tp must be 1..8 and 0 <= tp_rank < tp");
     if (o.tp > 1 && (m.n_kv_heads % o.tp || m.n_heads % o.tp || (m.ffn / o.tp) % 64 || m.ffn % o.tp || (m.vocab / o.tp) % 8 || m.vocab % o.tp))

@@ -33,6 +33,40 @@ cudaError_t launch_gather_rows(const void* x, const int32_t* rows, void* out, in
     return launch_k(gather_rows_kernel, dim3(n), dim3(128), 0, s, reinterpret_cast<const uint4*>(x), rows, reinterpret_cast<uint4*>(out), H / 8);
 }
 
+// fp8 row quantiser: per row, s = w8_row_scale(max |x|) and q = e4m3(x * (1/s)) — exact division by a power of two, then RNE, saturating.
+// One CTA per row; the second pass re-reads the row from L1 / L2.
+__global__ void __launch_bounds__(256) quant_rows_e4m3_kernel(const uint4* __restrict__ x, uint2* __restrict__ q, float* __restrict__ scale, int C8) {
+    griddep_launch(); griddep_wait();
+    const uint4* xr = x + (size_t)blockIdx.x * C8;
+    float amax = 0.f;
+    for (int i = threadIdx.x; i < C8; i += blockDim.x) {
+        float f[8];
+        unpack_bf16x8(xr[i], f);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(f[k]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    __shared__ float red[8];
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = amax;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < 8; ++w) amax = fmaxf(amax, red[w]);
+    const float s = w8_row_scale(amax), inv = 1.0f / s;
+    if (threadIdx.x == 0) scale[blockIdx.x] = s;
+    uint2* qr = q + (size_t)blockIdx.x * C8;
+    for (int i = threadIdx.x; i < C8; i += blockDim.x) {
+        float f[8];
+        unpack_bf16x8(xr[i], f);
+        qr[i] = pack_e4m3x8(f, inv);
+    }
+}
+cudaError_t launch_quant_rows_e4m3(const void* x, uint8_t* q, float* scale, int R, int C, cudaStream_t s) {
+    if (R <= 0) return cudaSuccess;
+    if (C <= 0 || C % 16 != 0) return cudaErrorInvalidValue;
+    return launch_k(quant_rows_e4m3_kernel, dim3(R), dim3(256), 0, s, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint2*>(q), scale, C / 8);
+}
+
 // y = x * rsqrt(mean(x^2) + eps) * g ; fp32 statistics, bf16 in/out.  Row cached in registers (H <= 8192).
 template <int VPT>   // uint4 vectors per thread, 256 threads
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ x, const uint4* __restrict__ g, uint4* __restrict__ y,

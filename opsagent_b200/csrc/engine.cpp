@@ -30,6 +30,7 @@ namespace oa {
 
 static thread_local std::string g_last_error;
 static int fail(int code, const std::string& msg) { g_last_error = msg; return code; }
+int fail_host(int code, const std::string& msg) { return fail(code, msg); }      // host-only entry points (capi_kernels.cpp)
 
 // selects `dev` on the calling thread for a scope and restores what was current before (the CUDA current device is per thread)
 struct CallerDevice {
@@ -282,16 +283,16 @@ public:
 
     std::string stats_json() {
         std::lock_guard<std::mutex> lk(mu_);
-        char b[1280];
+        char b[1408];
         std::snprintf(b, sizeof b,
                       "{\"requests_completed\": %llu, \"prefill_tokens\": %llu, \"decode_tokens\": %llu, \"prefill_steps\": %llu, "
                       "\"decode_steps\": %llu, \"preemptions\": %llu, \"pages_total\": %d, \"pages_free\": %zu, \"running\": %zu, "
                       "\"waiting\": %zu, \"kernel_launches\": %llu, \"h2d_bytes\": %llu, \"d2h_bytes\": %llu, \"weight_bytes\": %zu, "
-                      "\"kv_pool_bytes\": %zu, \"kv_cache_dtype\": \"%s\", \"busy_ms\": %.3f, \"prefix_hit_tokens\": %llu, \"pages_cached\": %zu, \"admissions_deferred\": %llu, \"mixed_steps\": %llu, \"cancelled\": %llu, \"grammar_states_computed\": %llu}",
+                      "\"kv_pool_bytes\": %zu, \"kv_cache_dtype\": \"%s\", \"weight_dtype\": \"%s\", \"busy_ms\": %.3f, \"prefix_hit_tokens\": %llu, \"pages_cached\": %zu, \"admissions_deferred\": %llu, \"mixed_steps\": %llu, \"cancelled\": %llu, \"grammar_states_computed\": %llu}",
                       (unsigned long long)n_completed_, (unsigned long long)n_prefill_tokens_, (unsigned long long)n_decode_tokens_,
                       (unsigned long long)n_prefill_steps_, (unsigned long long)n_decode_steps_, (unsigned long long)n_preempt_,
                       model_.num_pages, available_pages_locked(), running_.size(), waiting_.size(), (unsigned long long)launches_total(),
-                      (unsigned long long)model_.h2d_bytes, (unsigned long long)model_.d2h_bytes, model_.weight_bytes, model_.kv_pool_bytes, model_.cfg.kv_cache_dtype.c_str(), busy_ms_, (unsigned long long)n_prefix_hit_tokens_, cached_.size(),
+                      (unsigned long long)model_.h2d_bytes, (unsigned long long)model_.d2h_bytes, model_.weight_bytes, model_.kv_pool_bytes, model_.cfg.kv_cache_dtype.c_str(), model_.cfg.weight_dtype.c_str(), busy_ms_, (unsigned long long)n_prefix_hit_tokens_, cached_.size(),
                       (unsigned long long)n_admit_deferred_, (unsigned long long)n_mixed_steps_, (unsigned long long)n_cancelled_, (unsigned long long)n_mask_states_);
         return b;
     }
@@ -301,11 +302,11 @@ public:
                       "{\"model\": \"%s\", \"hidden\": %d, \"n_layers\": %d, \"n_heads\": %d, \"n_kv_heads\": %d, \"head_dim\": %d, \"ffn\": %d, "
                       "\"vocab\": %d, \"tie_embeddings\": %d, \"qkv_bias\": %d, \"rope_scaling\": %d, \"rope_theta\": %.1f, \"rms_eps\": %g, "
                       "\"template\": \"%s\", \"seed\": %llu, \"num_pages\": %d, \"page_size\": 64, \"max_seq_len\": %d, \"max_batch\": %d, "
-                      "\"sm_count\": %d, \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu, \"tp\": %d, \"tp_nvls\": %d%s}",
+                      "\"sm_count\": %d, \"decode_weight_bytes\": %.0f, \"kv_bytes_per_token\": %zu, \"tp\": %d, \"tp_nvls\": %d%s%s}",
                       c.name.c_str(), c.hidden, c.n_layers, c.n_heads, c.n_kv_heads, c.head_dim, c.ffn, c.vocab, c.tie_embeddings, c.qkv_bias,
                       c.rope_scaling, c.rope_theta, c.rms_eps, c.chat_template.c_str(), (unsigned long long)c.seed, model_.num_pages,
                       opt_.max_seq_len, opt_.max_batch, model_.sm_count, c.decode_weight_bytes(), c.kv_bytes_per_token(), opt_.tp, (model_.comm && model_.comm->nvls()) ? 1 : 0,
-                      c.kv_fp8() ? ", \"kv_cache_dtype\": \"fp8_e4m3\"" : "");
+                      c.kv_fp8() ? ", \"kv_cache_dtype\": \"fp8_e4m3\"" : "", c.w_fp8() ? ", \"weight_dtype\": \"fp8_e4m3\"" : "");
         return b;
     }
     bool serves_model(const std::string& name) const {
@@ -799,7 +800,8 @@ int oa_debug_kernel_times(oa_engine* h, char* buf, size_t n, int32_t reset) {
     if (!h || !buf) return fail(OA_ERR_BAD_REQUEST, "null argument");
     DeviceModel& m = h->e->model();
     std::string s = "{";
-    for (int i = 0; i < 14; ++i) {
+    const int n_ids = m.cfg.w_fp8() ? 15 : 14;          // fp8 weights: + the projection-input quantiser ("fp8_quant")
+    for (int i = 0; i < n_ids; ++i) {
         char t[128]; std::snprintf(t, sizeof t, "%s\"%s\": [%.4f, %ld]", i ? ", " : "", DeviceModel::kt_name(i), m.kt_ms[i], m.kt_n[i]); s += t;
         if (reset) { m.kt_ms[i] = 0; m.kt_n[i] = 0; }
     }

@@ -3,6 +3,7 @@
 //               a STAGES-deep shared-memory ring (128-byte swizzle), completion on `full` mbarriers;
 //   warps 0-7 : two consumer warpgroups; warpgroup g issues wgmma 64 x BN x 16 (bf16 -> fp32 in registers) for rows [64g, 64g + 64) of
 //               each 128-row A tile and releases ring slots (`empty`) as their MMAs retire.
+// fp8 (e4m3) operands (RingCfg FP8): the same bytes per unit hold 128 K elements; wgmma 64 x BN x 32, promoted to fp32 per unit.
 // Shared memory: [ring][accumulator region][barriers], 1024-byte aligned (the 128-byte swizzle atom).
 #pragma once
 #include "common.cuh"
@@ -20,10 +21,13 @@ static constexpr int RASTER_GROUP_M = 16;
 static constexpr int SMEM_LIMIT = 232448;                           // opt-in shared memory of one CTA on sm_90
 static constexpr int RING_SLACK = 1024 /*align*/ + 256 /*barriers*/;
 
-// ring of STAGES units (MT A tiles + one B tile each) next to an accumulator region of ACC bytes (default: the fp32 tile [MT * 128][BN])
-template <int BN_, int MT_, int STAGES_, int ACC = MT_ * BLOCK_M * BN_ * 4>
+// ring of STAGES units (MT A tiles + one B tile each) next to an accumulator region of ACC bytes (default: the fp32 tile [MT * 128][BN]).
+// A unit is one 128-byte swizzle row of K: 64 bf16 elements, or 128 e4m3 elements when FP8 (same bytes, same ring geometry).
+template <int BN_, int MT_, int STAGES_, int ACC = MT_ * BLOCK_M * BN_ * 4, bool FP8_ = false>
 struct RingCfg {
     static constexpr int BN = BN_, MT = MT_, STAGES = STAGES_;
+    static constexpr bool FP8 = FP8_;
+    static constexpr int KE = FP8 ? 2 * BLOCK_K : BLOCK_K;        // K elements per unit
     static constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;        // 16 KB
     static constexpr int A_BYTES = MT * A_TILE_BYTES;
     static constexpr int B_BYTES = BN * BLOCK_K * 2;
@@ -103,10 +107,13 @@ OA_DEVINL void ring_produce(const Ring& r, const CUtensorMap* tmA, const CUtenso
     }
 }
 
+template <class Cfg>
+OA_DEVINL void wg_mma_run_e4m3(float (&d)[Cfg::MT][Cfg::BN / 2], const Ring& r, int& s, uint32_t& ph, int n_kb);
 // Consumer side of the ring: n_kb units into this warpgroup's registers (rows [64g, 64g + 64) of each of the MT 128-row A tiles).
 // One wgmma group stays in flight; a slot is released (one arrival per consumer warp) once the group that read it has retired.
 template <class Cfg>
 OA_DEVINL void wg_mma_run(float (&d)[Cfg::MT][Cfg::BN / 2], const Ring& r, int& s, uint32_t& ph, int n_kb) {
+    if constexpr (Cfg::FP8) { wg_mma_run_e4m3<Cfg>(d, r, s, ph, n_kb); return; }
     constexpr int BN = Cfg::BN;
     const uint32_t g_off = (threadIdx.x >> 7) * 64 * 128;
     const bool leader = (threadIdx.x & 31) == 0;
@@ -138,6 +145,61 @@ OA_DEVINL void wg_mma_run(float (&d)[Cfg::MT][Cfg::BN / 2], const Ring& r, int& 
     }
     wgmma_wait<0>();
     if (prev >= 0 && leader) mbar_arrive(&r.empty_bar[prev]);
+}
+// e4m3 operands: a unit is 128 K elements, four k32 wgmmas per 128-column half.  They go into a zero-initialised fragment that is then
+// added to d in fp32 registers ("promotion": the fp8 tensor-core accumulator keeps only about 14 mantissa bits, so a long K is never summed
+// there).  Each group is retired before its sum is promoted, so its slot is released at once; the producer keeps the ring full meanwhile.
+// The temporary is 64 columns wide (32 registers): a 64 x 128 one leaves the fused finishers too few registers.
+template <class Cfg>
+OA_DEVINL void wg_mma_run_e4m3(float (&d)[Cfg::MT][Cfg::BN / 2], const Ring& r, int& s, uint32_t& ph, int n_kb) {
+    constexpr int BN = Cfg::BN, NW = BN > 64 ? 64 : BN;
+    const uint32_t g_off = (threadIdx.x >> 7) * 64 * 128;
+    const bool leader = (threadIdx.x & 31) == 0;
+    for (int i = 0; i < n_kb; ++i) {
+        mbar_wait(&r.full_bar[s], ph);
+        const uint32_t st = smem_u32(r.smem) + (uint32_t)(s * Cfg::STAGE_BYTES);
+        const uint64_t db = gmma_desc_sw128(st + (uint32_t)Cfg::A_BYTES);
+#pragma unroll
+        for (int m = 0; m < Cfg::MT; ++m) {
+            const uint64_t da = gmma_desc_sw128(st + (uint32_t)(m * Cfg::A_TILE_BYTES) + g_off);
+#pragma unroll
+            for (int nb = 0; nb < BN / NW; ++nb) {
+                float t[NW / 2] = {};
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_e4m3<NW>(t, da + (uint64_t)(k * 2), db + (uint64_t)(nb * NW * 8 + k * 2), k > 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<0>();
+#pragma unroll
+                for (int j = 0; j < NW / 2; ++j) d[m][nb * (NW / 2) + j] += t[j];
+            }
+        }
+        if (leader) mbar_arrive(&r.empty_bar[s]);
+        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
+    }
+}
+// fp8: d[row][col] *= s_a[row] * s_b[col], rows from row0 (the first of the MT 128-row tiles), columns from col0; rows >= M and columns
+// >= N get 0 (their TMA boxes were zero-filled).  s_a is written by the quantiser that precedes the GEMM, hence the dependency wait.
+template <int BN, int MT>
+OA_DEVINL void wg_scale_frag(float (&d)[MT][BN / 2], const W8Scales& w8, int row0, int col0, int M, int N) {
+    griddep_wait();
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3, g = threadIdx.x >> 7;
+#pragma unroll
+    for (int m = 0; m < MT; ++m) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = row0 + m * BLOCK_M + g * 64 + 16 * w + (lane >> 2) + 8 * h;
+            const float sa = row < M ? __ldg(w8.a + row) : 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = col0 + 8 * j + 2 * (lane & 3);          // even, and N % 8 == 0: both columns or neither are in range
+                const float2 sb = col < N ? __ldg(reinterpret_cast<const float2*>(w8.b + col)) : make_float2(0.f, 0.f);
+                d[m][4 * j + 2 * h] *= sa * sb.x;
+                d[m][4 * j + 2 * h + 1] *= sa * sb.y;
+                if ((j & 3) == 3) asm volatile("" ::: "memory");       // four loads in flight at a time: the scales never compete with d for registers
+            }
+        }
+    }
 }
 // registers -> the shared accumulator tile [MT * 128][BN], then one arrival per consumer warp on `bar`
 template <int BN, int MT>

@@ -5,6 +5,7 @@
 // tile in shared memory (`acc_full`), from which warpgroup 0 runs the epilogue, one output row per thread (bias | residual add | SwiGLU |
 // fp32 logits + row arg-max).  Decode (M <= 128) is weight-streaming and HBM-bound: B tiles are fetched with an evict-first L2 policy,
 // the small A operand with evict-last.  K tails and M/N tails rely on TMA zero fill + predicated stores.
+// FP8 instantiations (weight_dtype fp8_e4m3): e4m3 A and B with per-row fp32 scales, applied as a fragment enters the shared fp32 tile.
 //
 // The role of this file in the reference's terms: it is the arithmetic that sits behind
 // llms.OpenAIClient.Chat (reference pkg/llms/openai.go:69-104) once the `local-cuda` provider replaces the
@@ -17,31 +18,33 @@
 
 namespace oa {
 
-template <int BN>
-using GemmCfg = RingCfg<BN, 1, BN >= 256 ? 2 : 4>;      // the fp32 tile shares the 227 KB with the ring; one CTA per SM at every width
+// the fp32 tile shares the 227 KB with the ring; one CTA per SM at every width.  FP8: e4m3 operands (same bytes per unit, twice the K)
+template <int BN, bool FP8 = false>
+using GemmCfg = RingCfg<BN, 1, BN >= 256 ? 2 : 4, BLOCK_M * BN * 4, FP8>;
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool FP8 = false>
 __global__ void OA_GEMM_REGS gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                       const __grid_constant__ CUtensorMap tmB,
                                                                       const GemmParams p) {
-    using Cfg = GemmCfg<BN>;
+    using Cfg = GemmCfg<BN, FP8>;
     extern __shared__ uint8_t smem_raw[];
     const Ring ring = ring_setup<Cfg>(smem_raw, &tmA, &tmB);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     int n_blk, m_blk;
     raster_tile((int)blockIdx.x, (p.M + BLOCK_M - 1) / BLOCK_M, (p.N + BN - 1) / BN, m_blk, n_blk);
-    const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+    const int num_kb = (p.K + Cfg::KE - 1) / Cfg::KE;
 
     if (warp >= PRODUCER_WARP) {
         if (warp == PRODUCER_WARP && lane == 0) {
-            auto unit = [&](int kb, int& kx, int& a_row, int& b_row) { kx = kb * BLOCK_K; a_row = m_blk * BLOCK_M; b_row = n_blk * BN; };
+            auto unit = [&](int kb, int& kx, int& a_row, int& b_row) { kx = kb * Cfg::KE; a_row = m_blk * BLOCK_M; b_row = n_blk * BN; };
             ring_produce<Cfg, true>(ring, &tmA, &tmB, num_kb, unit, kEvictLast, kEvictFirst);
         }
     } else if (warp < CONSUMER_WARPS) {
         float d[1][BN / 2] = {};
         int s = 0; uint32_t ph = 0;
         wg_mma_run<Cfg>(d, ring, s, ph, num_kb);
+        if constexpr (FP8) wg_scale_frag<BN, 1>(d, p.w8, m_blk * BLOCK_M, n_blk * BN, p.M, p.N);
         float* acc = ring.acc;
         wg_acc_publish<BN, 1>(acc, d, ring.acc_full);
         if (warp >= 4) return;
@@ -130,10 +133,10 @@ __global__ void OA_GEMM_REGS gemm_wgmma_kernel(const __grid_constant__ CUtensorM
 
 int gemm_n_tiles(int N, int block_n) { return (N + block_n - 1) / block_n; }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool FP8 = false>
 static cudaError_t launch_one(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, cudaStream_t stream) {
     const dim3 grid(((p.N + BN - 1) / BN) * ((p.M + BLOCK_M - 1) / BLOCK_M));
-    return launch_gemm_kernel<gemm_wgmma_kernel<BN, EPI>>(grid, GemmCfg<BN>::SMEM_BYTES, stream, *tmA, *tmB, p);
+    return launch_gemm_kernel<gemm_wgmma_kernel<BN, EPI, FP8>>(grid, GemmCfg<BN, FP8>::SMEM_BYTES, stream, *tmA, *tmB, p);
 }
 
 template <int BN>
@@ -146,18 +149,45 @@ static cudaError_t launch_bn(const CUtensorMap* tmA, const CUtensorMap* tmB, con
     }
     return cudaErrorInvalidValue;
 }
+// fp8 operands: the projections' epilogues only (the LM head stays bf16), N tiles up to 128 (the promoted fragment's registers)
+template <int BN>
+static cudaError_t launch_bn_fp8(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, int epi, cudaStream_t s) {
+    switch (epi) {
+        case EPI_STORE: return launch_one<BN, EPI_STORE, true>(tmA, tmB, p, s);
+        case EPI_RESID: return launch_one<BN, EPI_RESID, true>(tmA, tmB, p, s);
+        case EPI_SWIGLU: return launch_one<BN, EPI_SWIGLU, true>(tmA, tmB, p, s);
+    }
+    return cudaErrorInvalidValue;
+}
 
 static bool persistent_disabled();
 static constexpr int PERSIST_BN = 128;      // 64 accumulator registers per consumer thread: no spills, and a 4-deep ring next to the 64 KB tile
 static int sm_count_cached();
 static long long persistent_min_tiles();
-template <int EPI>
+template <int EPI, bool FP8 = false>
 static cudaError_t launch_persistent(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, cudaStream_t stream);
 
 cudaError_t launch_gemm(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, int epilogue, int block_n,
                         cudaStream_t stream) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0 || (p.N % 8) != 0 || (p.K % 8) != 0) return cudaErrorInvalidValue;
     if (epilogue == EPI_SWIGLU && (p.N % 32) != 0) return cudaErrorInvalidValue;
+    if (p.w8.a || p.w8.b) {
+        if (!p.w8.a || !p.w8.b || (p.K % 16) != 0 || epilogue == EPI_LOGITS) return cudaErrorInvalidValue;
+        if (block_n == PERSIST_BN && !persistent_disabled() &&
+            (long long)((p.N + PERSIST_BN - 1) / PERSIST_BN) * ((p.M + BLOCK_M - 1) / BLOCK_M) >= persistent_min_tiles()) {
+            switch (epilogue) {
+                case EPI_STORE: return launch_persistent<EPI_STORE, true>(tmA, tmB, p, stream);
+                case EPI_RESID: return launch_persistent<EPI_RESID, true>(tmA, tmB, p, stream);
+                case EPI_SWIGLU: return launch_persistent<EPI_SWIGLU, true>(tmA, tmB, p, stream);
+            }
+        }
+        switch (block_n) {
+            case 32: return launch_bn_fp8<32>(tmA, tmB, p, epilogue, stream);
+            case 64: return launch_bn_fp8<64>(tmA, tmB, p, epilogue, stream);
+            case 128: return launch_bn_fp8<128>(tmA, tmB, p, epilogue, stream);
+        }
+        return cudaErrorInvalidValue;
+    }
     // large-M (prefill) shapes with the persistent kernel's tile go to it (epilogue overlapped with the next tile); tmB's box is block_n rows
     if (block_n == PERSIST_BN && epilogue != EPI_LOGITS && !persistent_disabled() &&
         (long long)((p.N + PERSIST_BN - 1) / PERSIST_BN) * ((p.M + BLOCK_M - 1) / BLOCK_M) >= persistent_min_tiles()) {
@@ -180,13 +210,13 @@ cudaError_t launch_gemm(const CUtensorMap* tmA, const CUtensorMap* tmB, const Ge
 // persistent tile GEMM (prefill, M > 128): one CTA per SM loops over 128 x 128 tiles in grouped raster order; warpgroup 1 runs the
 // wgmma main loop of tile i+1 while warpgroup 0 stores tile i.
 // =============================================================================================
-using PersistCfg = GemmCfg<PERSIST_BN>;
+using PersistCfg = GemmCfg<PERSIST_BN>;      // (the fp8 ring has the same bytes)
 
-template <int EPI>
+template <int EPI, bool FP8 = false>
 __global__ void OA_GEMM_REGS gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                             const __grid_constant__ CUtensorMap tmB,
                                                                             const GemmParams p) {
-    using Cfg = PersistCfg;
+    using Cfg = GemmCfg<PERSIST_BN, FP8>;
     constexpr int BN = Cfg::BN;
     extern __shared__ uint8_t smem_raw[];
     const Ring ring = ring_setup<Cfg>(smem_raw, &tmA, &tmB);
@@ -194,7 +224,7 @@ __global__ void OA_GEMM_REGS gemm_persistent_kernel(const __grid_constant__ CUte
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_tiles = (p.N + BN - 1) / BN, m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
     const int total_tiles = n_tiles * m_tiles;
-    const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+    const int num_kb = (p.K + Cfg::KE - 1) / Cfg::KE;
 
     if (warp >= PRODUCER_WARP) {
         if (warp == PRODUCER_WARP && lane == 0) {
@@ -203,7 +233,7 @@ __global__ void OA_GEMM_REGS gemm_persistent_kernel(const __grid_constant__ CUte
             int t = blockIdx.x, kb = 0, m_blk = 0, n_blk = 0;
             if (t < total_tiles) raster_tile(t, m_tiles, n_tiles, m_blk, n_blk);
             auto unit = [&](int, int& kx, int& a_row, int& b_row) {
-                kx = kb * BLOCK_K; a_row = m_blk * BLOCK_M; b_row = n_blk * BN;
+                kx = kb * Cfg::KE; a_row = m_blk * BLOCK_M; b_row = n_blk * BN;
                 if (++kb == num_kb) { kb = 0; t += gridDim.x; if (t < total_tiles) raster_tile(t, m_tiles, n_tiles, m_blk, n_blk); }
             };
             const int my_tiles = ((int)blockIdx.x < total_tiles) ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
@@ -214,13 +244,14 @@ __global__ void OA_GEMM_REGS gemm_persistent_kernel(const __grid_constant__ CUte
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
             float d[1][BN / 2] = {};
             wg_mma_run<Cfg>(d, ring, s, ph, num_kb);
+            int m_blk, n_blk; raster_tile(t, m_tiles, n_tiles, m_blk, n_blk);
+            if constexpr (FP8) wg_scale_frag<BN, 1>(d, p.w8, m_blk * BLOCK_M, n_blk * BN, p.M, p.N);
             mbar_wait(ring.acc_empty, (it & 1) ^ 1);      // the epilogue has drained the previous tile
             wg_acc_publish<BN, 1>(acc, d, ring.acc_full);
             if (warp >= 4) continue;
             // ---------------- epilogue: warpgroup 0 ----------------
             const int q = warp & 3;
             griddep_wait();
-            int m_blk, n_blk; raster_tile(t, m_tiles, n_tiles, m_blk, n_blk);
             mbar_wait(ring.acc_full, it & 1);
             const int row_base = m_blk * BLOCK_M + q * 32;
 #pragma unroll 1
@@ -274,18 +305,18 @@ static int sm_count_cached() {
     return n;
 }
 
-template <int EPI>
+template <int EPI, bool FP8>
 static cudaError_t launch_persistent(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, cudaStream_t stream) {
     const int tiles = ((p.N + PersistCfg::BN - 1) / PersistCfg::BN) * ((p.M + BLOCK_M - 1) / BLOCK_M);
     const int grid = tiles < sm_count_cached() ? tiles : sm_count_cached();
-    return launch_gemm_kernel<gemm_persistent_kernel<EPI>>(dim3(grid), PersistCfg::SMEM_BYTES, stream, *tmA, *tmB, p);
+    return launch_gemm_kernel<gemm_persistent_kernel<EPI, FP8>>(dim3(grid), PersistCfg::SMEM_BYTES, stream, *tmA, *tmB, p);
 }
 
 // =============================================================================================
 // stream-K (decode, M <= 128): persistent CTAs, balanced weight streaming, fp32 partials
 // =============================================================================================
-template <int BN, int MT>     // MT = 128-row tiles of A per unit (1: M <= 128, 2: M <= 256)
-using SkCfg = RingCfg<BN, MT, ring_stages_fit(BN, MT, 6)>;
+template <int BN, int MT, bool FP8 = false>     // MT = 128-row tiles of A per unit (1: M <= 128, 2: M <= 256)
+using SkCfg = RingCfg<BN, MT, ring_stages_fit(BN, MT, 6), MT * BLOCK_M * BN * 4, FP8>;
 
 // Epilogues finished INSIDE the stream-K GEMM by the CTA that holds a tile's first k-block (FUSE != 0): it adds the other CTAs' published
 // pieces to its own accumulator in CTA order (the stand-alone consumers' order: bit-identical sums) and writes the final bf16 result.
@@ -294,8 +325,9 @@ using SkCfg = RingCfg<BN, MT, ring_stages_fit(BN, MT, 6)>;
 //   FUSE 3  qkv     : (+ bias) -> bf16 -> RoPE -> q_out / paged K rows; V rows copied
 struct SkFuse {
     uint16_t* act; int F; unsigned int* tile_flags;
-    uint16_t* x; int ldx; int N;        // FUSE 2 (N = logical output columns; also the bound of FUSE 3)
+    uint16_t* x; int ldx; int N;        // FUSE 2 (N = logical output columns; also the bound of FUSE 3 and of the fp8 column scales)
     SkRopeArgs rope;                    // FUSE 3
+    W8Scales w8;                        // fp8 operands
 };
 
 // The fused finisher protocol.  Pieces of a tile live in CTAs c_first..c_last (sk_tile_ctas).  The CTA holding the FIRST k-block finishes
@@ -327,11 +359,11 @@ OA_DEVINL void sk_publish_piece(const StreamK& sk, const float* acc_s, long long
     if (threadIdx.x == EPI_WARP0 * 32) atomicAdd(flag, 1u);
 }
 
-template <int BN, int MT, int FUSE = 0>
+template <int BN, int MT, int FUSE = 0, bool FP8 = false>
 __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                          const __grid_constant__ CUtensorMap tmB, const int M,
                                                                          const StreamK sk, const SkFuse fz) {
-    using Cfg = SkCfg<BN, MT>;
+    using Cfg = SkCfg<BN, MT, FP8>;
     extern __shared__ uint8_t smem_raw[];
     const Ring ring = ring_setup<Cfg>(smem_raw, &tmA, &tmB);
     float* acc_s = ring.acc;                          // accumulator tile [MT * 128][BN]
@@ -346,7 +378,7 @@ __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtenso
             auto unit = [&](int i, int& kx, int& a_row, int& b_row) {
                 const long long u = u0 + i;
                 const int tile = (int)(u / sk.kb), kblk = (int)(u - (long long)tile * sk.kb);
-                kx = kblk * BLOCK_K; a_row = 0; b_row = tile * BN;
+                kx = kblk * Cfg::KE; a_row = 0; b_row = tile * BN;
             };
             ring_produce<Cfg, true>(ring, &tmA, &tmB, (int)(u1 - u0), unit, kEvictLast, kEvictFirst, sk.l2_prefetch_units);
         }
@@ -357,6 +389,7 @@ __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtenso
             const long long uend = min(u1, (long long)(tile + 1) * sk.kb);
             float d[MT][BN / 2] = {};
             wg_mma_run<Cfg>(d, ring, s, ph, (int)(uend - u));
+            if constexpr (FP8) wg_scale_frag<BN, MT>(d, fz.w8, 0, tile * BN, M, fz.N);
             mbar_wait(ring.acc_empty, (seg & 1) ^ 1);      // the epilogue has drained the previous segment
             wg_acc_publish<BN, MT>(acc_s, d, ring.acc_full);
             if (warp >= 4) { u = uend; continue; }
@@ -506,8 +539,9 @@ __global__ void OA_GEMM_REGS gemm_streamk_kernel(const __grid_constant__ CUtenso
     }
 }
 
-StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows) {
-    StreamK sk{}; sk.ws = ws; sk.bn = bn; sk.rows = rows > 128 ? 256 : 128; sk.kb = (K + BLOCK_K - 1) / BLOCK_K; sk.n_tiles = (N + bn - 1) / bn;
+StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows, bool fp8) {
+    const int ke = fp8 ? 2 * BLOCK_K : BLOCK_K;
+    StreamK sk{}; sk.ws = ws; sk.bn = bn; sk.rows = rows > 128 ? 256 : 128; sk.kb = (K + ke - 1) / ke; sk.n_tiles = (N + bn - 1) / bn;
     sk.total = (long long)sk.n_tiles * sk.kb; sk.G = (int)std::min<long long>(G, sk.total);
     sk.l2_prefetch_units = 0;
     return sk;
@@ -516,36 +550,46 @@ size_t streamk_ws_bytes(int N, int bn, int G, int rows) { return (size_t)(G + (N
 
 template <int BN, int MT, int FUSE = 0>
 static cudaError_t launch_sk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, const StreamK& sk, cudaStream_t stream, SkFuse fz = SkFuse{}) {
+    if (fz.w8.a) {
+        // fp8: one row tile and N <= 128 only, and no fused SwiGLU.  With the promotion temporary, a second 64 x 128 fragment (MT = 2) or the
+        // SwiGLU finisher's chunk buffers exceed the 168 registers per thread (ptxas spills); those shapes take the tile kernel / the consumer.
+        if constexpr (BN <= 128 && MT == 1 && FUSE != 1)
+            return launch_gemm_kernel<gemm_streamk_kernel<BN, MT, FUSE, true>>(dim3(sk.G), SkCfg<BN, MT, true>::SMEM_BYTES, stream, *tmA, *tmB, M, sk, fz);
+        return cudaErrorInvalidValue;
+    }
     return launch_gemm_kernel<gemm_streamk_kernel<BN, MT, FUSE>>(dim3(sk.G), SkCfg<BN, MT>::SMEM_BYTES, stream, *tmA, *tmB, M, sk, fz);
 }
+// fp8: both scale arrays or neither, K in whole 16-byte TMA rows
+static bool w8_bad(const W8Scales& w8, int K) { return (w8.a == nullptr) != (w8.b == nullptr) || (w8.a && (K % 16) != 0); }
 cudaError_t launch_gemm_streamk_swiglu(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int F, int K, const StreamK& sk, void* act,
-                                       unsigned int* tile_flags, cudaStream_t stream) {
-    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (F % 16) != 0 || (K % 8) != 0 || !act || !tile_flags) return cudaErrorInvalidValue;
+                                       unsigned int* tile_flags, cudaStream_t stream, W8Scales w8) {
+    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (F % 16) != 0 || (K % 8) != 0 || !act || !tile_flags || w8_bad(w8, K)) return cudaErrorInvalidValue;
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;      // finishing CTAs wait for publishing CTAs: all must be resident
-    SkFuse fz{}; fz.act = reinterpret_cast<uint16_t*>(act); fz.F = F; fz.tile_flags = tile_flags;
+    SkFuse fz{}; fz.act = reinterpret_cast<uint16_t*>(act); fz.F = F; fz.tile_flags = tile_flags; fz.N = 2 * F; fz.w8 = w8;
     return launch_sk<128, 1, 1>(tmA, tmB, M, sk, stream, fz);
 }
 cudaError_t launch_gemm_streamk_resid(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, void* x, int ldx,
-                                      unsigned int* tile_flags, cudaStream_t stream) {
-    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (N % 32) != 0 || (K % 8) != 0 || !x || !tile_flags || (ldx % 8) != 0) return cudaErrorInvalidValue;
+                                      unsigned int* tile_flags, cudaStream_t stream, W8Scales w8) {
+    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (N % 32) != 0 || (K % 8) != 0 || !x || !tile_flags || (ldx % 8) != 0 || w8_bad(w8, K)) return cudaErrorInvalidValue;
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;      // finishing CTAs wait for publishing CTAs: all must be resident
-    SkFuse fz{}; fz.tile_flags = tile_flags; fz.x = reinterpret_cast<uint16_t*>(x); fz.ldx = ldx; fz.N = N;
+    SkFuse fz{}; fz.tile_flags = tile_flags; fz.x = reinterpret_cast<uint16_t*>(x); fz.ldx = ldx; fz.N = N; fz.w8 = w8;
     return launch_sk<128, 1, 2>(tmA, tmB, M, sk, stream, fz);
 }
 cudaError_t launch_gemm_streamk_rope(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, const SkRopeArgs& rope,
-                                     unsigned int* tile_flags, cudaStream_t stream) {
-    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (K % 8) != 0 || !tile_flags) return cudaErrorInvalidValue;
+                                     unsigned int* tile_flags, cudaStream_t stream, W8Scales w8) {
+    if (M <= 0 || M > BLOCK_M || sk.rows != 128 || sk.bn != 128 || (K % 8) != 0 || !tile_flags || w8_bad(w8, K)) return cudaErrorInvalidValue;
     if ((rope.D != 64 && rope.D != 128) || N != (rope.nh + 2 * rope.nkv) * rope.D) return cudaErrorInvalidValue;      // BN must be a multiple of D; chunks of 32 never straddle a head
     if (sk.G > sm_count_cached()) return cudaErrorInvalidValue;
-    SkFuse fz{}; fz.tile_flags = tile_flags; fz.N = N; fz.rope = rope;
+    SkFuse fz{}; fz.tile_flags = tile_flags; fz.N = N; fz.rope = rope; fz.w8 = w8;
     return launch_sk<128, 1, 3>(tmA, tmB, M, sk, stream, fz);
 }
-cudaError_t launch_gemm_streamk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, cudaStream_t stream) {
-    if (M <= 0 || M > sk.rows || (N % 8) != 0 || (K % 8) != 0) return cudaErrorInvalidValue;
-    if (sk.rows == 256) return sk.bn == 128 ? launch_sk<128, 2>(tmA, tmB, M, sk, stream) : cudaErrorInvalidValue;
-    if (sk.bn == 256) return launch_sk<256, 1>(tmA, tmB, M, sk, stream);
-    if (sk.bn == 128) return launch_sk<128, 1>(tmA, tmB, M, sk, stream);      // more CTAs than SMs run in waves: the plain kernel never waits on another CTA
-    if (sk.bn == 64) return launch_sk<64, 1>(tmA, tmB, M, sk, stream);       // half the partial bytes again; per-projection opt-in (sk_bn_o / sk_bn_down / sk_bn_qkv)
+cudaError_t launch_gemm_streamk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, cudaStream_t stream, W8Scales w8) {
+    if (M <= 0 || M > sk.rows || (N % 8) != 0 || (K % 8) != 0 || w8_bad(w8, K)) return cudaErrorInvalidValue;
+    SkFuse fz{}; fz.N = N; fz.w8 = w8;
+    if (sk.rows == 256) return sk.bn == 128 ? launch_sk<128, 2>(tmA, tmB, M, sk, stream, fz) : cudaErrorInvalidValue;
+    if (sk.bn == 256) return launch_sk<256, 1>(tmA, tmB, M, sk, stream, fz);      // bf16 only
+    if (sk.bn == 128) return launch_sk<128, 1>(tmA, tmB, M, sk, stream, fz);      // more CTAs than SMs run in waves: the plain kernel never waits on another CTA
+    if (sk.bn == 64) return launch_sk<64, 1>(tmA, tmB, M, sk, stream, fz);       // half the partial bytes again; per-projection opt-in (sk_bn_o / sk_bn_down / sk_bn_qkv)
     return cudaErrorInvalidValue;
 }
 

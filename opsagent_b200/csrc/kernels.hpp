@@ -23,6 +23,9 @@ enum GemmEpilogue : int {
     EPI_SWIGLU = 2,   // out[M,N/2] bf16 = silu(gate)*up, B rows interleaved 16 gate / 16 up
     EPI_LOGITS = 3,   // per-row (max, argmax) partial per N-tile -> argmax_ws; optional fp32 logits store
 };
+// fp8 (e4m3) operands: A[M,K] and B[N,K] hold bytes, and C[m,n] = a[m] * b[n] * sum_k A[m,k] B[n,k] with the fp32 row scales a[M], b[N]
+// (the quantiser below).  Both null: bf16 operands.
+struct W8Scales { const float* a; const float* b; };
 struct GemmParams {
     int M, N, K;
     void* out; int ldo;             // bf16 output, leading dimension in elements
@@ -33,8 +36,10 @@ struct GemmParams {
     // grammar-constrained rows (EPI_LOGITS): row r with mask_slot[r] >= 0 takes its arg-max only over the token ids whose bit is set in
     // mask_table[mask_slot[r] * mask_words ...]; bit index = col_offset + column (col_offset: first global id of a vocab-parallel shard)
     const uint32_t* mask_table; const int32_t* mask_slot; int mask_words, col_offset;
+    W8Scales w8;                    // fp8 operands (EPI_STORE / EPI_RESID / EPI_SWIGLU, block_n <= 128)
 };
-// tmA: box {64, 128} over A[M,K]; tmB: box {64, block_n} over B[N,K].  block_n in {32,64,128,256}.
+// tmA: box {64, 128} over A[M,K]; tmB: box {64, block_n} over B[N,K].  block_n in {32,64,128,256}.  fp8: byte maps (make_tmap_u8_2d) with
+// boxes {128, 128} and {128, block_n}.
 cudaError_t launch_gemm(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p, int epilogue, int block_n,
                         cudaStream_t stream);
 int gemm_n_tiles(int N, int block_n);
@@ -47,7 +52,7 @@ struct StreamK {
     float* ws; int bn, kb, n_tiles, G, rows; long long total;  // rows = 128 or 256 accumulator rows per slot      // kb = k blocks per tile, total = n_tiles * kb, G = CTAs
     int l2_prefetch_units;                                    // weight tiles each CTA prefetches into L2 before griddepcontrol.wait
 };
-StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows = 128);
+StreamK make_streamk(float* ws, int N, int K, int bn, int G, int rows = 128, bool fp8 = false);   // fp8: 128-wide k blocks
 // CTA c owns units [c*total/G, (c+1)*total/G), so unit u lives in CTA floor(((u+1)*G - 1) / total): the CTAs holding the first and the
 // last k-block of `tile`.  One definition for the kernels, the consumers and the host plan (32-bit products: host-checked per model).
 #ifdef __CUDACC__
@@ -60,11 +65,13 @@ inline void sk_tile_ctas(const StreamK& sk, uint32_t tile, uint32_t& c_first, ui
 }
 
 size_t streamk_ws_bytes(int N, int bn, int G, int rows = 128);
-cudaError_t launch_gemm_streamk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, cudaStream_t stream);
+// every stream-K launcher takes fp8 operands with non-null w8 scales (sk from make_streamk(..., fp8 = true); BN <= 128)
+cudaError_t launch_gemm_streamk(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, cudaStream_t stream,
+                                W8Scales w8 = {});
 // gate/up projection with the SwiGLU finished inside the GEMM (BN=128, one row tile): act[M,F] = silu(gate)*up, bit-identical to
 // launch_gemm_streamk + launch_sk_swiglu.  tile_flags: >= n_tiles counters, zero between launches (the kernel re-arms them).
 cudaError_t launch_gemm_streamk_swiglu(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int F, int K, const StreamK& sk, void* act,
-                                       unsigned int* tile_flags, cudaStream_t stream);
+                                       unsigned int* tile_flags, cudaStream_t stream, W8Scales w8 = {});
 // x[T,H] (bf16, in place) += sum of partials; xn = rmsnorm(x) * gain
 cudaError_t launch_sk_resid_rmsnorm(const StreamK& sk, void* x, const void* gain, void* xn, int T, int H, float eps, cudaStream_t s);
 // act[T,F] = silu(gate) * up from the interleaved gate/up partials (N = 2F)
@@ -78,11 +85,11 @@ struct SkRopeArgs {       // q/k/v from the qkv projection's partials (+ bias): 
 // o / down projection with the residual add finished inside the GEMM: x[M, ldx] (bf16, in place) += A.B^T, bit-identical to
 // launch_gemm_streamk + the sum/residual half of launch_sk_resid_rmsnorm.  Follow with launch_rmsnorm_wide for the norm.
 cudaError_t launch_gemm_streamk_resid(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, void* x, int ldx,
-                                      unsigned int* tile_flags, cudaStream_t stream);
+                                      unsigned int* tile_flags, cudaStream_t stream, W8Scales w8 = {});
 // qkv projection with bias + RoPE + the paged-KV write finished inside the GEMM (no qkv tensor, no consumer launch), bit-identical to
 // launch_gemm_streamk + launch_sk_rope_kv_write
 cudaError_t launch_gemm_streamk_rope(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, const StreamK& sk, const SkRopeArgs& rope,
-                                     unsigned int* tile_flags, cudaStream_t stream);
+                                     unsigned int* tile_flags, cudaStream_t stream, W8Scales w8 = {});
 // ---- cluster split-K GEMM for projections with few output tiles (gemm_clusterk.cu): S CTAs of one cluster own one 128-column tile and 1/S
 // of K each, reduce through distributed shared memory and finish the epilogue together (no partial workspace, no consumer launch) ----
 int clusterk_pick(int N, int K, int sms, int min_fill_pct = 80);        // cluster size for this shape (8, 4, 3, 2) or 0 = keep the stream-K path
@@ -102,6 +109,9 @@ cudaError_t launch_embed_gather(const int32_t* ids, const void* table, void* out
 cudaError_t launch_rmsnorm(const void* x, const void* gain, void* y, int T, int H, float eps, cudaStream_t s);
 // gather rows: out[i,:] = x[rows[i],:]
 cudaError_t launch_gather_rows(const void* x, const int32_t* rows, void* out, int n, int H, cudaStream_t s);
+// fp8 (e4m3) rows: x bf16 [R, C] -> q [R, C] bytes + scale [R] fp32, per row s = w8_row_scale(amax) and q = e4m3(x / s) (round to nearest
+// even, saturating).  Weights at load time and every projection input of the fp8-weight forward.  C % 16 == 0.
+cudaError_t launch_quant_rows_e4m3(const void* x, uint8_t* q, float* scale, int R, int C, cudaStream_t s);
 // RoPE (HF rotate_half pairing) on q and k in `qkv` [T, (nh+2nkv)*D]; rotated q -> q_out [T, nh*D];
 // rotated k and v -> paged KV cache rows.  slot[t] = page*page_size + offset of token t.
 struct KvLayout {

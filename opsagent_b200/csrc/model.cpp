@@ -30,13 +30,22 @@ void* DeviceModel::dmalloc(size_t bytes) {
 void DeviceModel::make_weight_maps(WeightMat& w) {
     const int bns[4] = {32, 64, 128, 256};
     for (int i = 0; i < 4; ++i) {
-        int r = make_tmap_bf16_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint64_t)w.K, (uint32_t)bns[i], 64);
+        int r = w.fp8 ? make_tmap_u8_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint32_t)bns[i], 128)
+                      : make_tmap_bf16_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint64_t)w.K, (uint32_t)bns[i], 64);
         if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for a weight matrix (code " + std::to_string(r) + ")");
     }
 }
-void DeviceModel::alloc_weight(WeightMat& w, int N, int K) {
-    w.N = N; w.K = K; w.ptr = dmalloc((size_t)N * K * 2); weight_bytes += (size_t)N * K * 2;
+void DeviceModel::alloc_weight(WeightMat& w, int N, int K, bool fp8) {
+    w.N = N; w.K = K; w.fp8 = fp8;
+    if (fp8) {
+        w.ptr = dmalloc((size_t)N * K); w.sw = reinterpret_cast<float*>(dmalloc((size_t)N * 4)); weight_bytes += (size_t)N * K + (size_t)N * 4;
+    } else {
+        w.ptr = dmalloc((size_t)N * K * 2); weight_bytes += (size_t)N * K * 2;
+    }
     make_weight_maps(w);
+}
+void DeviceModel::quantise_weight(WeightMat& w, const void* bf16) {
+    cuda_check(launch_quant_rows_e4m3(bf16, reinterpret_cast<uint8_t*>(w.ptr), w.sw, w.N, w.K, stream), "quantise weights (fp8)");
 }
 
 // Build the RoPE table exactly as oracle/llama_ref.c:oa_ref_rope_table does (double math, then cast).
@@ -95,17 +104,27 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     if (cfg.tie_embeddings) { lm_head.ptr = reinterpret_cast<uint16_t*>(embed) + (size_t)r * V_l * H; lm_head.N = V_l; lm_head.K = H; make_weight_maps(lm_head); }
     else { alloc_weight(lm_head, V_l, H); cuda_check(launch_init_weight(lm_head.ptr, cfg.seed, (uint64_t)L * 16 + TG_LMHEAD, -1, V_l, H, cfg.init_std, 0.f, stream, r * V_l), "init lm_head"); }
     layers.resize(L);
+    // fp8 projections: each matrix is generated (or loaded) as bf16 into one scratch the size of the largest, then quantised into its e4m3
+    // allocation on the same stream; the scratch is freed once the weights are in place, so the peak stays below the bf16 engine's weights
+    const bool w8 = cfg.w_fp8();
+    if (w8) w8_scratch_ = dmalloc(std::max({(size_t)qkvd * H, (size_t)H * qd, (size_t)2 * F * H, (size_t)H * F}) * 2);
+    auto bf16_of = [&](const WeightMat& w) { return reinterpret_cast<uint16_t*>(w8 ? w8_scratch_ : w.ptr); };
+    auto finish = [&](WeightMat& w) { if (w8) quantise_weight(w, w8_scratch_); };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l]; const uint64_t b = (uint64_t)l * 16;
-        alloc_weight(ly.qkv, qkvd, H); alloc_weight(ly.o, H, qd); alloc_weight(ly.gu, 2 * F, H); alloc_weight(ly.down, H, F);
-        uint16_t* wq = reinterpret_cast<uint16_t*>(ly.qkv.ptr);
+        alloc_weight(ly.qkv, qkvd, H, w8); alloc_weight(ly.o, H, qd, w8); alloc_weight(ly.gu, 2 * F, H, w8); alloc_weight(ly.down, H, F, w8);
+        uint16_t* wq = bf16_of(ly.qkv);
         // column-parallel q|k|v and gate|up (row shards), row-parallel o and down (column shards of the logical tensors)
         cuda_check(launch_init_weight(wq, cfg.seed, b + T_WQ, -1, qd, H, cfg.init_std, 0.f, stream, r * qd), "init wq");
         cuda_check(launch_init_weight(wq + (size_t)qd * H, cfg.seed, b + T_WK, -1, kd, H, cfg.init_std, 0.f, stream, r * kd), "init wk");
         cuda_check(launch_init_weight(wq + (size_t)(qd + kd) * H, cfg.seed, b + T_WV, -1, kd, H, cfg.init_std, 0.f, stream, r * kd), "init wv");
-        cuda_check(launch_init_weight(ly.o.ptr, cfg.seed, b + T_WO, -1, H, qd, cfg.init_std, 0.f, stream, 0, r * qd, qd_g), "init wo");
-        cuda_check(launch_init_weight(ly.gu.ptr, cfg.seed, b + T_WG, (int64_t)(b + T_WU), 2 * (int64_t)F, H, cfg.init_std, 0.f, stream, r * F), "init wgu");
-        cuda_check(launch_init_weight(ly.down.ptr, cfg.seed, b + T_WD, -1, H, F, cfg.init_std, 0.f, stream, 0, r * F, F_g), "init wd");
+        finish(ly.qkv);
+        cuda_check(launch_init_weight(bf16_of(ly.o), cfg.seed, b + T_WO, -1, H, qd, cfg.init_std, 0.f, stream, 0, r * qd, qd_g), "init wo");
+        finish(ly.o);
+        cuda_check(launch_init_weight(bf16_of(ly.gu), cfg.seed, b + T_WG, (int64_t)(b + T_WU), 2 * (int64_t)F, H, cfg.init_std, 0.f, stream, r * F), "init wgu");
+        finish(ly.gu);
+        cuda_check(launch_init_weight(bf16_of(ly.down), cfg.seed, b + T_WD, -1, H, F, cfg.init_std, 0.f, stream, 0, r * F, F_g), "init wd");
+        finish(ly.down);
         ly.ln1 = dmalloc((size_t)H * 2); ly.ln2 = dmalloc((size_t)H * 2);
         cuda_check(launch_init_weight(ly.ln1, cfg.seed, b + T_LN1, -1, 1, H, nstd, 1.f, stream), "init ln1");
         cuda_check(launch_init_weight(ly.ln2, cfg.seed, b + T_LN2, -1, 1, H, nstd, 1.f, stream), "init ln2");
@@ -120,6 +139,11 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
 
     kv_k_scale.assign(L, 1.0f); kv_v_scale.assign(L, 1.0f);
     if (!opt.weights.empty()) load_checkpoint(opt.weights);
+    if (w8_scratch_) {
+        cuda_check(cudaStreamSynchronize(stream), "weight quantisation");
+        cuda_check(cudaFree(w8_scratch_), "cudaFree");
+        allocs_.erase(std::find(allocs_.begin(), allocs_.end(), w8_scratch_)); w8_scratch_ = nullptr;
+    }
 
     // ---- RoPE table ----
     {
@@ -144,6 +168,15 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
         if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for an activation buffer (code " + std::to_string(r) + ")");
     };
     amap(&tm_xn_, xn_, MR, H); amap(&tm_attn_, attn_, MR, qd); amap(&tm_act_, act_, MR, F);
+    if (w8) {      // e4m3 copies of the projection inputs with one fp32 scale per row (zeroed: the GEMMs' stale rows stay finite)
+        auto q8 = [&](uint8_t*& p, float*& sc, CUtensorMap* tm, int cols) {
+            p = reinterpret_cast<uint8_t*>(dmalloc((size_t)MR * cols)); sc = reinterpret_cast<float*>(dmalloc((size_t)MR * 4));
+            cuda_check(cudaMemsetAsync(p, 0, (size_t)MR * cols, stream), "memset"); cuda_check(cudaMemsetAsync(sc, 0, (size_t)MR * 4, stream), "memset");
+            int r = make_tmap_u8_2d(tm, p, (uint64_t)MR, (uint64_t)cols, 128, 128);
+            if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for an fp8 activation buffer (code " + std::to_string(r) + ")");
+        };
+        q8(xn8_, sxn_, &tm_xn8_, H); q8(attn8_, sattn_, &tm_attn8_, qd); q8(act8_, sact_, &tm_act8_, F);
+    }
     cuda_check(cudaMemsetAsync(q_, 0, (size_t)MR * qd * 2, stream), "memset");
     // sampled rows (debug logits sample every row of a short prefill: up to 2048)
     const int MS = max_sample_;
@@ -277,6 +310,9 @@ static void load_kv_scales(const SafeTensors& st, int L, std::vector<float>& ks,
 }
 
 void DeviceModel::load_checkpoint(const std::string& path) {
+    // the seeded init (and, with fp8 weights, its quantisation through the scratch) is still queued on `stream`, which the synchronous copies
+    // below do not wait for
+    cuda_check(cudaStreamSynchronize(stream), "weight init");
     SafeTensors st(path);
     const int H = cfg.hidden, L = cfg.n_layers, D = cfg.head_dim, V = cfg.vocab;
     const int qd = nh_l * D, kd = nkv_l * D;
@@ -284,12 +320,18 @@ void DeviceModel::load_checkpoint(const std::string& path) {
     std::vector<uint16_t> buf;
     // every tensor must have exactly the logical shape [R, C] (vectors: [C]) this model configuration implies — a transposed, truncated or
     // wrong-config (hidden / ffn / heads / vocab) checkpoint is refused with a message instead of being read out of bounds
+    const bool w8 = cfg.w_fp8();
     auto checked = [&](const std::string& name, int64_t R, int64_t C) -> const StTensor& {
         const StTensor& t = st.get(name);
         const bool ok = (t.shape.size() == 2 && t.shape[0] == R && t.shape[1] == C) || (R == 1 && t.shape.size() == 1 && t.shape[0] == C);
         if (!ok) {
             std::string got = "["; for (size_t i = 0; i < t.shape.size(); ++i) got += (i ? ", " : "") + std::to_string(t.shape[i]); got += "]";
             throw std::runtime_error("checkpoint tensor " + name + " has shape " + got + ", this model needs [" + (R == 1 ? "" : std::to_string(R) + ", ") + std::to_string(C) + "]");
+        }
+        const bool proj = name.size() > 12 && name.compare(name.size() - 12, 12, "_proj.weight") == 0;     // q/k/v/o/gate/up/down
+        if (proj && t.dtype == "F8_E4M3") {
+            if (!w8) throw std::runtime_error("checkpoint tensor " + name + " is F8_E4M3: fp8 projection weights need weight_dtype fp8_e4m3");
+            return t;
         }
         if (t.dtype != "BF16" && t.dtype != "F16" && t.dtype != "F32") throw std::runtime_error("checkpoint tensor " + name + " has unsupported dtype " + t.dtype);
         return t;       // SafeTensors already verified bytes == prod(shape) * sizeof(dtype)
@@ -303,17 +345,91 @@ void DeviceModel::load_checkpoint(const std::string& path) {
         cuda_check(cudaMemcpy(dst, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
     };
     if (cfg.kv_fp8()) load_kv_scales(st, L, kv_k_scale, kv_v_scale);
+    // fp8 weights (tp == 1): projection w is assembled from whole checkpoint rows, rows[i] = (tensor name, its row count, source row) of
+    // physical row i.  bf16 / F16 / F32 parts are quantised on the device with the row rule; F8_E4M3 parts (compressed-tensors "FP8"
+    // checkpoints) bring their bytes and `<name>_scale` (per row [N, 1] / [N], or per tensor [] / [1]).  One matrix takes one kind.
+    // Static activation scales (`input_scale`) are not read: activations are quantised per token at run time.
+    struct SrcRow { const std::string* name; int64_t R, row; };
+    auto load_proj8 = [&](WeightMat& w, const std::vector<SrcRow>& rows) {
+        const int64_t K = w.K;
+        int n_f8 = 0;
+        for (const SrcRow& sr : rows) n_f8 += checked(*sr.name, sr.R, K).dtype == "F8_E4M3";
+        if (n_f8 == 0) {
+            std::vector<uint16_t> hb((size_t)w.N * K);
+            for (size_t i = 0; i < rows.size(); ++i) to_bf16_rows(st.get(*rows[i].name), K, rows[i].row, 0, K, hb.data() + i * K);
+            // on `stream`: a pageable cudaMemcpy may return before its DMA lands, and it does not order with a non-blocking stream
+            cuda_check(cudaMemcpyAsync(w8_scratch_, hb.data(), hb.size() * 2, cudaMemcpyHostToDevice, stream), "checkpoint H2D");
+            quantise_weight(w, w8_scratch_);
+            cuda_check(cudaStreamSynchronize(stream), "weight quantisation");
+            return;
+        }
+        if (n_f8 != (int)rows.size()) throw std::runtime_error("checkpoint tensor " + *rows[0].name + ": the parts of one fused projection (q/k/v, gate/up) must all be F8_E4M3 or none");
+        std::vector<uint8_t> hq((size_t)w.N * K); std::vector<float> hs((size_t)w.N);
+        std::map<std::string, std::vector<float>> scales;
+        for (size_t i = 0; i < rows.size(); ++i) {
+            const std::string& nm = *rows[i].name;
+            std::vector<float>& sc = scales[nm];
+            if (sc.empty()) {
+                const std::string sn = nm + "_scale";
+                if (!st.has(sn)) throw std::runtime_error("checkpoint tensor " + nm + " is F8_E4M3 but " + sn + " is missing");
+                const StTensor& t = st.get(sn);
+                const int64_t R = rows[i].R;
+                const bool per_row = (t.shape.size() == 2 && t.shape[0] == R && t.shape[1] == 1) || (t.shape.size() == 1 && t.shape[0] == R);
+                const bool per_tensor = t.shape.empty() || (t.shape.size() == 1 && t.shape[0] == 1) || (t.shape.size() == 2 && t.shape[0] == 1 && t.shape[1] == 1);
+                if (!per_row && !per_tensor) throw std::runtime_error("checkpoint tensor " + sn + " must have shape [" + std::to_string(R) + ", 1], [" + std::to_string(R) + "], [] or [1]");
+                const int64_t n = per_row ? R : 1;
+                sc.resize((size_t)R);
+                for (int64_t j = 0; j < n; ++j) {
+                    float v;
+                    if (t.dtype == "F32") std::memcpy(&v, t.data + 4 * j, 4);
+                    else if (t.dtype == "BF16") { uint16_t b; std::memcpy(&b, t.data + 2 * j, 2); const uint32_t u = (uint32_t)b << 16; std::memcpy(&v, &u, 4); }
+                    else if (t.dtype == "F16") { uint16_t b; std::memcpy(&b, t.data + 2 * j, 2); v = f16_bits_to_f32(b); }
+                    else throw std::runtime_error("checkpoint tensor " + sn + " has unsupported dtype " + t.dtype);
+                    if (!std::isfinite(v) || v <= 0.f) throw std::runtime_error("checkpoint tensor " + sn + " must be finite and > 0");
+                    sc[(size_t)j] = v;
+                }
+                if (!per_row) std::fill(sc.begin(), sc.end(), sc[0]);
+            }
+            std::memcpy(hq.data() + i * K, st.get(nm).data + (size_t)rows[i].row * K, (size_t)K);
+            hs[i] = sc[(size_t)rows[i].row];
+        }
+        cuda_check(cudaMemcpyAsync(w.ptr, hq.data(), hq.size(), cudaMemcpyHostToDevice, stream), "checkpoint H2D");
+        cuda_check(cudaMemcpyAsync(w.sw, hs.data(), hs.size() * 4, cudaMemcpyHostToDevice, stream), "checkpoint H2D");
+        cuda_check(cudaStreamSynchronize(stream), "checkpoint H2D");
+    };
     slice("model.embed_tokens.weight", V, H, 0, V, 0, H, embed);
     slice("model.norm.weight", 1, H, 0, 1, 0, H, final_norm);
     if (!cfg.tie_embeddings) slice(st.has("lm_head.weight") ? "lm_head.weight" : "model.embed_tokens.weight", V, H, r * V_l, V_l, 0, H, lm_head.ptr);
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l]; const std::string p = "model.layers." + std::to_string(l) + ".";
+        if (w8) {
+            const std::string nq = p + "self_attn.q_proj.weight", nk = p + "self_attn.k_proj.weight", nv = p + "self_attn.v_proj.weight";
+            const std::string no = p + "self_attn.o_proj.weight", ng = p + "mlp.gate_proj.weight", nu = p + "mlp.up_proj.weight", nd = p + "mlp.down_proj.weight";
+            std::vector<SrcRow> rq;
+            for (int64_t i = 0; i < qd; ++i) rq.push_back({&nq, qd, i});
+            for (int64_t i = 0; i < kd; ++i) rq.push_back({&nk, kd, i});
+            for (int64_t i = 0; i < kd; ++i) rq.push_back({&nv, kd, i});
+            load_proj8(ly.qkv, rq);
+            std::vector<SrcRow> ro, rg, rd;
+            for (int64_t i = 0; i < H; ++i) { ro.push_back({&no, H, i}); rd.push_back({&nd, H, i}); }
+            for (int64_t blk = 0; blk < F_l / 16; ++blk)
+                for (int64_t w = 0; w < 32; ++w) rg.push_back({w < 16 ? &ng : &nu, F_l, blk * 16 + (w & 15)});      // 16 gate rows, 16 up rows
+            load_proj8(ly.o, ro); load_proj8(ly.gu, rg); load_proj8(ly.down, rd);
+        } else {
         uint16_t* wq = reinterpret_cast<uint16_t*>(ly.qkv.ptr);
         slice(p + "self_attn.q_proj.weight", cfg.q_dim(), H, r * qd, qd, 0, H, wq);
         slice(p + "self_attn.k_proj.weight", cfg.kv_dim(), H, r * kd, kd, 0, H, wq + (size_t)qd * H);
         slice(p + "self_attn.v_proj.weight", cfg.kv_dim(), H, r * kd, kd, 0, H, wq + (size_t)(qd + kd) * H);
         slice(p + "self_attn.o_proj.weight", H, cfg.q_dim(), 0, H, r * qd, qd, ly.o.ptr);
         slice(p + "mlp.down_proj.weight", H, cfg.ffn, 0, H, r * F_l, F_l, ly.down.ptr);
+        // gate/up: physical rows interleaved in blocks of 16 (16 gate rows, 16 up rows)
+        const StTensor& tg = checked(p + "mlp.gate_proj.weight", cfg.ffn, H); const StTensor& tu = checked(p + "mlp.up_proj.weight", cfg.ffn, H);
+        buf.resize((size_t)2 * F_l * H);
+        for (int64_t blk = 0; blk < F_l / 16; ++blk)
+            for (int64_t w = 0; w < 32; ++w)
+                to_bf16_rows(w < 16 ? tg : tu, H, r * F_l + blk * 16 + (w & 15), 0, H, buf.data() + (size_t)(blk * 32 + w) * H);
+        cuda_check(cudaMemcpy(ly.gu.ptr, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
+        }
         slice(p + "input_layernorm.weight", 1, H, 0, 1, 0, H, ly.ln1);
         slice(p + "post_attention_layernorm.weight", 1, H, 0, 1, 0, H, ly.ln2);
         if (cfg.qkv_bias) {
@@ -322,13 +438,6 @@ void DeviceModel::load_checkpoint(const std::string& path) {
             slice(p + "self_attn.k_proj.bias", 1, cfg.kv_dim(), 0, 1, r * kd, kd, bq + qd);
             slice(p + "self_attn.v_proj.bias", 1, cfg.kv_dim(), 0, 1, r * kd, kd, bq + qd + kd);
         }
-        // gate/up: physical rows interleaved in blocks of 16 (16 gate rows, 16 up rows)
-        const StTensor& tg = checked(p + "mlp.gate_proj.weight", cfg.ffn, H); const StTensor& tu = checked(p + "mlp.up_proj.weight", cfg.ffn, H);
-        buf.resize((size_t)2 * F_l * H);
-        for (int64_t blk = 0; blk < F_l / 16; ++blk)
-            for (int64_t w = 0; w < 32; ++w)
-                to_bf16_rows(w < 16 ? tg : tu, H, r * F_l + blk * 16 + (w & 15), 0, H, buf.data() + (size_t)(blk * 32 + w) * H);
-        cuda_check(cudaMemcpy(ly.gu.ptr, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
     }
 }
 
@@ -345,7 +454,7 @@ DeviceModel::~DeviceModel() {
 
 const char* DeviceModel::kt_name(int id) {
     static const char* n[16] = {"h2d+embed", "rmsnorm", "qkv_gemm", "rope_kv", "attention", "attn_merge", "o_gemm", "resid_rmsnorm", "gate_up_gemm",
-                                "swiglu", "down_gemm", "gather+norm", "lm_head", "argmax+d2h", "", ""};
+                                "swiglu", "down_gemm", "gather+norm", "lm_head", "argmax+d2h", "fp8_quant", ""};
     return n[id & 15];
 }
 void DeviceModel::sync() { cuda_check(cudaStreamSynchronize(stream), "stream sync"); }
@@ -482,14 +591,21 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
 
     size_t ek = 0;
     if (profile_all) {
-        if (ev_all.size() < (size_t)L * 12 + 16) { size_t o = ev_all.size(); ev_all.resize((size_t)L * 12 + 16); for (size_t i = o; i < ev_all.size(); ++i) cudaEventCreate(&ev_all[i]); }
+        const size_t n_ev = (size_t)L * (cfg.w_fp8() ? 16 : 12) + 16;      // fp8: four quantiser launches per layer
+        if (ev_all.size() < n_ev) { size_t o = ev_all.size(); ev_all.resize(n_ev); for (size_t i = o; i < ev_all.size(); ++i) cudaEventCreate(&ev_all[i]); }
         ev_ids.assign(ev_all.size(), 0);
         cudaEventRecord(ev_all[ek++], stream);
     }
     auto MARK = [&](int id) { if (profile_all && ek < ev_all.size()) { ev_ids[ek] = id; cudaEventRecord(ev_all[ek++], stream); } };
     const float scale_log2e = (1.0f / std::sqrt((float)D)) * 1.4426950408889634f;
     cuda_check(launch_embed_gather(d_tok, embed, x_, T, H, cfg.vocab, stream), "embed"); MARK(0);
-    const bool use_sk = opt.streamk && T <= std::min(256, std::max(128, opt.sk_max_rows));   // decode-sized batches (one or, opt-in, two 128-row tiles)
+    // fp8 weights: every projection reads its input as e4m3 rows + per-row scales, quantised by one kernel right before the GEMM
+    const bool w8 = cfg.w_fp8();
+    auto quant = [&](const void* x, uint8_t* q, float* sc, int C) { if (w8) { cuda_check(launch_quant_rows_e4m3(x, q, sc, T, C, stream), "fp8 quantise"); MARK(14); } };
+    const CUtensorMap *tA_xn = w8 ? &tm_xn8_ : &tm_xn_, *tA_attn = w8 ? &tm_attn8_ : &tm_attn_, *tA_act = w8 ? &tm_act8_ : &tm_act_;
+    auto w8s = [&](const float* sa, const WeightMat& w) { return w8 ? W8Scales{sa, w.sw} : W8Scales{}; };
+    // decode-sized batches (one or, opt-in, two 128-row tiles; fp8: one, the promoted fp8 fragment leaves no registers for a second)
+    const bool use_sk = opt.streamk && T <= (w8 ? 128 : std::min(256, std::max(128, opt.sk_max_rows)));
     const int sk_rows = T > 128 ? 256 : 128;
     auto attention = [&](int l) {
         if (profile_attn) cudaEventRecord(ev[2 * l], stream);
@@ -511,10 +627,13 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
     };
     if (use_sk) {
         // decode-sized batch: persistent stream-K projections (fp32 partials) + fused consumers
-        auto bn_of = [&](int o) { return sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_); };   // two row tiles need BN=128 (registers)
+        auto bn_of = [&](int o) {      // two row tiles (and fp8) need BN <= 128 (registers)
+            const int bn = sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_);
+            return w8 ? std::min(bn, 128) : bn;
+        };
         auto with_pf = [&](StreamK k) { k.l2_prefetch_units = std::max(0, opt.sk_l2_prefetch_kb * 1024 / (k.bn * 128)); return k; };
-        const StreamK sk_qkv = make_streamk(sk_ws_, qkvd, H, bn_of(opt.sk_bn_qkv), sk_G_, sk_rows), sk_o = make_streamk(sk_ws_, H, qd, bn_of(opt.sk_bn_o), sk_G_, sk_rows);
-        const StreamK sk_gu = make_streamk(sk_ws_, 2 * F, H, bn_of(opt.sk_bn_gu), sk_G_, sk_rows), sk_dn = make_streamk(sk_ws_, H, F, bn_of(opt.sk_bn_down), sk_G_, sk_rows);
+        const StreamK sk_qkv = make_streamk(sk_ws_, qkvd, H, bn_of(opt.sk_bn_qkv), sk_G_, sk_rows, w8), sk_o = make_streamk(sk_ws_, H, qd, bn_of(opt.sk_bn_o), sk_G_, sk_rows, w8);
+        const StreamK sk_gu = make_streamk(sk_ws_, 2 * F, H, bn_of(opt.sk_bn_gu), sk_G_, sk_rows, w8), sk_dn = make_streamk(sk_ws_, H, F, bn_of(opt.sk_bn_down), sk_G_, sk_rows, w8);
         cuda_check(launch_rmsnorm(x_, layers[0].ln1, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
         const StreamK pf_qkv = with_pf(sk_qkv), pf_o = with_pf(sk_o), pf_gu = with_pf(sk_gu), pf_dn = with_pf(sk_dn);
         // qkv / o / down epilogues finished inside the GEMM (same conditions as the fused SwiGLU; every projection at BN = 128, tile counts within the flag arrays)
@@ -526,28 +645,30 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         const int ck_qkv = (sk_rows == 128 && (opt.sk_clusterk & 1) && (D == 64 || D == 128)) ? clusterk_pick(qkvd, H, sm_count, opt.sk_clusterk_min_fill) : 0;
         const int ck_o = (sk_rows == 128 && (opt.sk_clusterk & 2) && !use_tp) ? clusterk_pick(H, qd, sm_count, opt.sk_clusterk_min_fill) : 0;
         const int ck_dn = (sk_rows == 128 && (opt.sk_clusterk & 4) && !use_tp) ? clusterk_pick(H, F, sm_count, opt.sk_clusterk_min_fill) : 0;
-        const bool fuse_swiglu = opt.sk_fuse_swiglu && sk_rows == 128 && sk_gu.bn == 128 && sk_G_ <= sm_count && sk_gu.n_tiles <= SK_MAX_FLAG_TILES;
+        const bool fuse_swiglu = opt.sk_fuse_swiglu && !w8 && sk_rows == 128 && sk_gu.bn == 128 && sk_G_ <= sm_count && sk_gu.n_tiles <= SK_MAX_FLAG_TILES;
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
+            quant(xn_, xn8_, sxn_, H);
             if (ck_qkv) {
                 cuda_check(launch_gemm_clusterk_rope(&tm_xn_, ly.qkv.map(128), T, qkvd, H, ck_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh), stream),
                            "qkv gemm + RoPE + KV write (cluster split-K)"); MARK(2);
             } else if (fuse_rope) {
-                cuda_check(launch_gemm_streamk_rope(&tm_xn_, ly.qkv.map(128), T, qkvd, H, pf_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh),
-                                                    tile_flags_ + 0 * SK_MAX_FLAG_TILES, stream), "qkv gemm + RoPE + KV write (stream-K)"); MARK(2);
+                cuda_check(launch_gemm_streamk_rope(tA_xn, ly.qkv.map(128), T, qkvd, H, pf_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh),
+                                                    tile_flags_ + 0 * SK_MAX_FLAG_TILES, stream, w8s(sxn_, ly.qkv)), "qkv gemm + RoPE + KV write (stream-K)"); MARK(2);
             } else {
-                cuda_check(launch_gemm_streamk(&tm_xn_, ly.qkv.map(sk_qkv.bn), T, qkvd, H, pf_qkv, stream), "qkv gemm (stream-K)"); MARK(2);
+                cuda_check(launch_gemm_streamk(tA_xn, ly.qkv.map(sk_qkv.bn), T, qkvd, H, pf_qkv, stream, w8s(sxn_, ly.qkv)), "qkv gemm (stream-K)"); MARK(2);
                 cuda_check(launch_sk_rope_kv_write(sk_qkv, ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope (stream-K)"); MARK(3);
             }
             attention(l);
+            quant(attn_, attn8_, sattn_, qd);
             if (ck_o) {
                 cuda_check(launch_gemm_clusterk_resid(&tm_attn_, ly.o.map(128), T, H, qd, ck_o, x_, H, stream), "o gemm + residual (cluster split-K)"); MARK(6);
                 cuda_check(launch_rmsnorm_wide(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(7);
             } else if (fuse_o) {
-                cuda_check(launch_gemm_streamk_resid(&tm_attn_, ly.o.map(128), T, H, qd, pf_o, x_, H, tile_flags_ + 1 * SK_MAX_FLAG_TILES, stream), "o gemm + residual (stream-K)"); MARK(6);
+                cuda_check(launch_gemm_streamk_resid(tA_attn, ly.o.map(128), T, H, qd, pf_o, x_, H, tile_flags_ + 1 * SK_MAX_FLAG_TILES, stream, w8s(sattn_, ly.o)), "o gemm + residual (stream-K)"); MARK(6);
                 cuda_check(launch_rmsnorm_wide(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(7);
             } else {
-            cuda_check(launch_gemm_streamk(&tm_attn_, ly.o.map(sk_o.bn), T, H, qd, pf_o, stream), "o gemm (stream-K)"); MARK(6);
+            cuda_check(launch_gemm_streamk(tA_attn, ly.o.map(sk_o.bn), T, H, qd, pf_o, stream, w8s(sattn_, ly.o)), "o gemm (stream-K)"); MARK(6);
             if (use_tp) {      // row-parallel projection: all-reduce the rank partials over NVLink peer memory, then residual + norm
                 const int b = comm->next_buffer();
                 const TpComm::Signal sg = comm->next_signal();     // "buffer written" handshake rides on the two kernels: no barrier launch
@@ -568,12 +689,14 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
             }
             MARK(7);
             }
+            quant(xn_, xn8_, sxn_, H);
             if (fuse_swiglu) {
                 cuda_check(launch_gemm_streamk_swiglu(&tm_xn_, ly.gu.map(128), T, F, H, pf_gu, act_, tile_flags_ + 2 * SK_MAX_FLAG_TILES, stream), "gate_up gemm + SwiGLU (stream-K)"); MARK(8);
             } else {
-                cuda_check(launch_gemm_streamk(&tm_xn_, ly.gu.map(sk_gu.bn), T, 2 * F, H, pf_gu, stream), "gate_up gemm (stream-K)"); MARK(8);
+                cuda_check(launch_gemm_streamk(tA_xn, ly.gu.map(sk_gu.bn), T, 2 * F, H, pf_gu, stream, w8s(sxn_, ly.gu)), "gate_up gemm (stream-K)"); MARK(8);
                 cuda_check(launch_sk_swiglu(sk_gu, act_, T, F, stream), "swiglu"); MARK(9);
             }
+            quant(act_, act8_, sact_, F);
             const void* next_gain = (l + 1 < L) ? layers[l + 1].ln1 : final_norm;
             if (ck_dn) {
                 cuda_check(launch_gemm_clusterk_resid(&tm_act_, ly.down.map(128), T, H, F, ck_dn, x_, H, stream), "down gemm + residual (cluster split-K)"); MARK(10);
@@ -581,11 +704,11 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 continue;
             }
             if (fuse_dn) {
-                cuda_check(launch_gemm_streamk_resid(&tm_act_, ly.down.map(128), T, H, F, pf_dn, x_, H, tile_flags_ + 3 * SK_MAX_FLAG_TILES, stream), "down gemm + residual (stream-K)"); MARK(10);
+                cuda_check(launch_gemm_streamk_resid(tA_act, ly.down.map(128), T, H, F, pf_dn, x_, H, tile_flags_ + 3 * SK_MAX_FLAG_TILES, stream, w8s(sact_, ly.down)), "down gemm + residual (stream-K)"); MARK(10);
                 cuda_check(launch_rmsnorm_wide(x_, next_gain, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(7);
                 continue;
             }
-            cuda_check(launch_gemm_streamk(&tm_act_, ly.down.map(sk_dn.bn), T, H, F, pf_dn, stream), "down gemm (stream-K)"); MARK(10);
+            cuda_check(launch_gemm_streamk(tA_act, ly.down.map(sk_dn.bn), T, H, F, pf_dn, stream, w8s(sact_, ly.down)), "down gemm (stream-K)"); MARK(10);
             if (use_tp) {
                 const int b = comm->next_buffer();
                 const TpComm::Signal sg = comm->next_signal();
@@ -617,15 +740,18 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 cuda_check(launch_ar_resid_bf16(comm->d_peer_sym(b), tp, x_, T, H, stream), "allreduce+resid");
             }
         };
-        const int bn_qkv = pick_bn(T, qkvd, opt.bn_qkv, false), bn_o = pick_bn(T, H, opt.bn_o, false);
-        const int bn_gu = pick_bn(T, 2 * F, opt.bn_gu, true), bn_down = pick_bn(T, H, opt.bn_down, false);
+        auto cap = [&](int bn) { return w8 ? std::min(bn, 128) : bn; };      // fp8 tiles are at most 128 wide (registers)
+        const int bn_qkv = cap(pick_bn(T, qkvd, opt.bn_qkv, false)), bn_o = cap(pick_bn(T, H, opt.bn_o, false));
+        const int bn_gu = cap(pick_bn(T, 2 * F, opt.bn_gu, true)), bn_down = cap(pick_bn(T, H, opt.bn_down, false));
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
             cuda_check(launch_rmsnorm(x_, ly.ln1, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
-            GemmParams g{}; g.M = T; g.N = qkvd; g.K = H; g.out = qkv_; g.ldo = qkvd; g.bias = ly.bqkv;
-            cuda_check(launch_gemm(&tm_xn_, ly.qkv.map(bn_qkv), g, EPI_STORE, bn_qkv, stream), "qkv gemm"); MARK(2);
+            quant(xn_, xn8_, sxn_, H);
+            GemmParams g{}; g.M = T; g.N = qkvd; g.K = H; g.out = qkv_; g.ldo = qkvd; g.bias = ly.bqkv; g.w8 = w8s(sxn_, ly.qkv);
+            cuda_check(launch_gemm(tA_xn, ly.qkv.map(bn_qkv), g, EPI_STORE, bn_qkv, stream), "qkv gemm"); MARK(2);
             cuda_check(launch_rope_kv_write(qkv_, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope"); MARK(3);
             attention(l);
+            quant(attn_, attn8_, sattn_, qd);
             if (use_tp) {      // bf16 partial -> symmetric buffer, barrier, x += sum over ranks (rank order)
                 const int b = comm->next_buffer();
                 GemmParams go{}; go.M = T; go.N = H; go.K = qd; go.out = comm->sym(b); go.ldo = H;
@@ -633,12 +759,14 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 cuda_check(comm->barrier(stream), "xgpu barrier");
                 allreduce_resid_bf16(b);
             } else {
-                GemmParams go{}; go.M = T; go.N = H; go.K = qd; go.out = x_; go.ldo = H; go.resid = x_; go.ldr = H;
-                cuda_check(launch_gemm(&tm_attn_, ly.o.map(bn_o), go, EPI_RESID, bn_o, stream), "o gemm"); MARK(6);
+                GemmParams go{}; go.M = T; go.N = H; go.K = qd; go.out = x_; go.ldo = H; go.resid = x_; go.ldr = H; go.w8 = w8s(sattn_, ly.o);
+                cuda_check(launch_gemm(tA_attn, ly.o.map(bn_o), go, EPI_RESID, bn_o, stream), "o gemm"); MARK(6);
             }
             cuda_check(launch_rmsnorm(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(1);
-            GemmParams gg{}; gg.M = T; gg.N = 2 * F; gg.K = H; gg.out = act_; gg.ldo = F;
-            cuda_check(launch_gemm(&tm_xn_, ly.gu.map(bn_gu), gg, EPI_SWIGLU, bn_gu, stream), "gate_up gemm"); MARK(8);
+            quant(xn_, xn8_, sxn_, H);
+            GemmParams gg{}; gg.M = T; gg.N = 2 * F; gg.K = H; gg.out = act_; gg.ldo = F; gg.w8 = w8s(sxn_, ly.gu);
+            cuda_check(launch_gemm(tA_xn, ly.gu.map(bn_gu), gg, EPI_SWIGLU, bn_gu, stream), "gate_up gemm"); MARK(8);
+            quant(act_, act8_, sact_, F);
             if (use_tp) {
                 const int b = comm->next_buffer();
                 GemmParams gd{}; gd.M = T; gd.N = H; gd.K = F; gd.out = comm->sym(b); gd.ldo = H;
@@ -646,8 +774,8 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 cuda_check(comm->barrier(stream), "xgpu barrier");
                 allreduce_resid_bf16(b);
             } else {
-                GemmParams gd{}; gd.M = T; gd.N = H; gd.K = F; gd.out = x_; gd.ldo = H; gd.resid = x_; gd.ldr = H;
-                cuda_check(launch_gemm(&tm_act_, ly.down.map(bn_down), gd, EPI_RESID, bn_down, stream), "down gemm"); MARK(10);
+                GemmParams gd{}; gd.M = T; gd.N = H; gd.K = F; gd.out = x_; gd.ldo = H; gd.resid = x_; gd.ldr = H; gd.w8 = w8s(sact_, ly.down);
+                cuda_check(launch_gemm(tA_act, ly.down.map(bn_down), gd, EPI_RESID, bn_down, stream), "down gemm"); MARK(10);
             }
         }
     }

@@ -13,6 +13,7 @@ namespace oa {
 
 struct WeightMat {
     void* ptr = nullptr; int N = 0, K = 0;
+    bool fp8 = false; float* sw = nullptr;      // fp8: ptr holds e4m3 bytes [N, K], sw the fp32 scale of each row (weight_dtype fp8_e4m3)
     CUtensorMap tm[4];            // B-operand maps for BLOCK_N = 32, 64, 128, 256
     const CUtensorMap* map(int bn) const { return &tm[bn == 32 ? 0 : bn == 64 ? 1 : bn == 128 ? 2 : 3]; }
 };
@@ -76,7 +77,8 @@ public:
     float *rope_cos = nullptr, *rope_sin = nullptr;
 
 private:
-    void alloc_weight(WeightMat& w, int N, int K);
+    void alloc_weight(WeightMat& w, int N, int K, bool fp8 = false);
+    void quantise_weight(WeightMat& w, const void* bf16);      // fp8: bf16 [N, K] on the device -> w's bytes and row scales (row rule)
     void load_checkpoint(const std::string& path);     // overwrite the seeded tensors with this rank's slices of an HF checkpoint
     void make_weight_maps(WeightMat& w);
     int pick_bn(int M, int N, int override_bn, bool swiglu) const;
@@ -85,6 +87,10 @@ private:
     // activations
     void *x_ = nullptr, *xn_ = nullptr, *qkv_ = nullptr, *q_ = nullptr, *attn_ = nullptr, *act_ = nullptr, *xs_ = nullptr, *xsn_ = nullptr;
     CUtensorMap tm_xn_, tm_attn_, tm_act_, tm_xsn_;
+    // fp8 weights: the projection inputs quantised per row (e4m3 bytes + fp32 scales), allocated only then
+    uint8_t *xn8_ = nullptr, *attn8_ = nullptr, *act8_ = nullptr; float *sxn_ = nullptr, *sattn_ = nullptr, *sact_ = nullptr;
+    CUtensorMap tm_xn8_, tm_attn8_, tm_act8_;
+    void* w8_scratch_ = nullptr;                   // bf16 staging of one projection while the weights are generated or loaded (then freed)
     float* amax_val_ = nullptr; int* amax_idx_ = nullptr; int32_t* d_out_ids_ = nullptr;
     uint32_t* mask_table_ = nullptr;               // [mask_slots][mask_words] allowed-token bitsets of grammar states (filled on demand by the scheduler)
     float *part_o_ = nullptr, *part_ml_ = nullptr; int max_part_slots_ = 0;

@@ -13,6 +13,8 @@ run memcheck_kernels 420 memcheck python -m pytest tests/test_kernels_gpu.py -x 
 run memcheck_engine 420 memcheck python -m pytest tests/test_engine_gpu.py -x -q -k "greedy_generation or concurrent_requests or grammar_constrained or prefix_cache or preemption or native_front_routes or cluster_splitk and not 1b"
 run memcheck_kv_fp8 420 memcheck python -m pytest tests/test_kv_fp8_gpu.py -x -q -k "fp8_paged or kv_write"
 run racecheck_kv_fp8 420 racecheck python -m pytest tests/test_kv_fp8_gpu.py -x -q -k "fp8_paged or kv_write"
+run memcheck_w8_fp8 420 memcheck python -m pytest tests/test_w8_fp8_gpu.py -x -q -k "quantiser or (gemm_fp8 and not long_k) and (-1-False or -7-False or quantiser)"
+run racecheck_w8_fp8 420 racecheck python -m pytest tests/test_w8_fp8_gpu.py -x -q -k "quantiser or (gemm_fp8 and not long_k) and (-1-False or -7-False or quantiser)"
 run racecheck_smoke 240 racecheck python -c "import __graft_entry__ as g; g.smoke()"
 run synccheck_smoke 240 synccheck python -c "import __graft_entry__ as g; g.smoke()"
 run initcheck_smoke 240 initcheck python -c "import __graft_entry__ as g; g.smoke()"
