@@ -1,6 +1,6 @@
 // model.cpp — see model.hpp.
 #include "model.hpp"
-#include "safetensors.hpp"
+#include "checkpoint.hpp"
 
 #include <algorithm>
 #include <cmath>
@@ -14,6 +14,9 @@ namespace oa {
 
 void cuda_check(cudaError_t e, const char* what) {
     if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
+}
+static void tmap_check(int r, const char* what) {
+    if (r != 0) throw std::runtime_error(std::string("cuTensorMapEncodeTiled failed for ") + what + " (code " + std::to_string(r) + ")");
 }
 
 // tensor ids of the seeded generator: layer*16 + kind; globals at layer index n_layers (oracle/llama_ref.c)
@@ -30,9 +33,8 @@ void* DeviceModel::dmalloc(size_t bytes) {
 void DeviceModel::make_weight_maps(WeightMat& w) {
     const int bns[4] = {32, 64, 128, 256};
     for (int i = 0; i < 4; ++i) {
-        int r = w.fp8 ? make_tmap_u8_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint32_t)bns[i], 128)
-                      : make_tmap_bf16_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint64_t)w.K, (uint32_t)bns[i], 64);
-        if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for a weight matrix (code " + std::to_string(r) + ")");
+        tmap_check(w.fp8 ? make_tmap_u8_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint32_t)bns[i], 128)
+                         : make_tmap_bf16_2d(&w.tm[i], w.ptr, (uint64_t)w.N, (uint64_t)w.K, (uint64_t)w.K, (uint32_t)bns[i], 64), "a weight matrix");
     }
 }
 void DeviceModel::alloc_weight(WeightMat& w, int N, int K, bool fp8) {
@@ -44,8 +46,8 @@ void DeviceModel::alloc_weight(WeightMat& w, int N, int K, bool fp8) {
     }
     make_weight_maps(w);
 }
-void DeviceModel::quantise_weight(WeightMat& w, const void* bf16) {
-    cuda_check(launch_quant_rows_e4m3(bf16, reinterpret_cast<uint8_t*>(w.ptr), w.sw, w.N, w.K, stream), "quantise weights (fp8)");
+void DeviceModel::commit(WeightMat& w) {
+    if (w.fp8) cuda_check(launch_quant_rows_e4m3(w8_scratch_, reinterpret_cast<uint8_t*>(w.ptr), w.sw, w.N, w.K, stream), "quantise weights (fp8)");
 }
 
 // Build the RoPE table exactly as oracle/llama_ref.c:oa_ref_rope_table does (double math, then cast).
@@ -108,23 +110,21 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     // allocation on the same stream; the scratch is freed once the weights are in place, so the peak stays below the bf16 engine's weights
     const bool w8 = cfg.w_fp8();
     if (w8) w8_scratch_ = dmalloc(std::max({(size_t)qkvd * H, (size_t)H * qd, (size_t)2 * F * H, (size_t)H * F}) * 2);
-    auto bf16_of = [&](const WeightMat& w) { return reinterpret_cast<uint16_t*>(w8 ? w8_scratch_ : w.ptr); };
-    auto finish = [&](WeightMat& w) { if (w8) quantise_weight(w, w8_scratch_); };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l]; const uint64_t b = (uint64_t)l * 16;
         alloc_weight(ly.qkv, qkvd, H, w8); alloc_weight(ly.o, H, qd, w8); alloc_weight(ly.gu, 2 * F, H, w8); alloc_weight(ly.down, H, F, w8);
-        uint16_t* wq = bf16_of(ly.qkv);
+        uint16_t* wq = bf16_dst(ly.qkv);
         // column-parallel q|k|v and gate|up (row shards), row-parallel o and down (column shards of the logical tensors)
         cuda_check(launch_init_weight(wq, cfg.seed, b + T_WQ, -1, qd, H, cfg.init_std, 0.f, stream, r * qd), "init wq");
         cuda_check(launch_init_weight(wq + (size_t)qd * H, cfg.seed, b + T_WK, -1, kd, H, cfg.init_std, 0.f, stream, r * kd), "init wk");
         cuda_check(launch_init_weight(wq + (size_t)(qd + kd) * H, cfg.seed, b + T_WV, -1, kd, H, cfg.init_std, 0.f, stream, r * kd), "init wv");
-        finish(ly.qkv);
-        cuda_check(launch_init_weight(bf16_of(ly.o), cfg.seed, b + T_WO, -1, H, qd, cfg.init_std, 0.f, stream, 0, r * qd, qd_g), "init wo");
-        finish(ly.o);
-        cuda_check(launch_init_weight(bf16_of(ly.gu), cfg.seed, b + T_WG, (int64_t)(b + T_WU), 2 * (int64_t)F, H, cfg.init_std, 0.f, stream, r * F), "init wgu");
-        finish(ly.gu);
-        cuda_check(launch_init_weight(bf16_of(ly.down), cfg.seed, b + T_WD, -1, H, F, cfg.init_std, 0.f, stream, 0, r * F, F_g), "init wd");
-        finish(ly.down);
+        commit(ly.qkv);
+        cuda_check(launch_init_weight(bf16_dst(ly.o), cfg.seed, b + T_WO, -1, H, qd, cfg.init_std, 0.f, stream, 0, r * qd, qd_g), "init wo");
+        commit(ly.o);
+        cuda_check(launch_init_weight(bf16_dst(ly.gu), cfg.seed, b + T_WG, (int64_t)(b + T_WU), 2 * (int64_t)F, H, cfg.init_std, 0.f, stream, r * F), "init wgu");
+        commit(ly.gu);
+        cuda_check(launch_init_weight(bf16_dst(ly.down), cfg.seed, b + T_WD, -1, H, F, cfg.init_std, 0.f, stream, 0, r * F, F_g), "init wd");
+        commit(ly.down);
         ly.ln1 = dmalloc((size_t)H * 2); ly.ln2 = dmalloc((size_t)H * 2);
         cuda_check(launch_init_weight(ly.ln1, cfg.seed, b + T_LN1, -1, 1, H, nstd, 1.f, stream), "init ln1");
         cuda_check(launch_init_weight(ly.ln2, cfg.seed, b + T_LN2, -1, 1, H, nstd, 1.f, stream), "init ln2");
@@ -158,24 +158,20 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     max_rows_ = std::max(opt.max_step_tokens, opt.max_batch);
     max_sample_ = std::max(opt.max_batch, std::min(max_rows_, 2048));
     const int MR = max_rows_;
-    x_ = dmalloc((size_t)MR * H * 2); xn_ = dmalloc((size_t)MR * H * 2); qkv_ = dmalloc((size_t)MR * qkvd * 2);
-    q_ = dmalloc((size_t)MR * qd * 2); attn_ = dmalloc((size_t)MR * qd * 2); act_ = dmalloc((size_t)MR * F * 2);
-    cuda_check(cudaMemsetAsync(xn_, 0, (size_t)MR * H * 2, stream), "memset");
-    cuda_check(cudaMemsetAsync(attn_, 0, (size_t)MR * qd * 2, stream), "memset");
-    cuda_check(cudaMemsetAsync(act_, 0, (size_t)MR * F * 2, stream), "memset");
+    x_ = dmalloc((size_t)MR * H * 2); qkv_ = dmalloc((size_t)MR * qkvd * 2); q_ = dmalloc((size_t)MR * qd * 2);
     auto amap = [&](CUtensorMap* tm, void* p, int rows, int cols) {
-        int r = make_tmap_bf16_2d(tm, p, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, 128, 64);
-        if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for an activation buffer (code " + std::to_string(r) + ")");
+        tmap_check(make_tmap_bf16_2d(tm, p, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, 128, 64), "an activation buffer");
     };
-    amap(&tm_xn_, xn_, MR, H); amap(&tm_attn_, attn_, MR, qd); amap(&tm_act_, act_, MR, F);
-    if (w8) {      // e4m3 copies of the projection inputs with one fp32 scale per row (zeroed: the GEMMs' stale rows stay finite)
-        auto q8 = [&](uint8_t*& p, float*& sc, CUtensorMap* tm, int cols) {
-            p = reinterpret_cast<uint8_t*>(dmalloc((size_t)MR * cols)); sc = reinterpret_cast<float*>(dmalloc((size_t)MR * 4));
-            cuda_check(cudaMemsetAsync(p, 0, (size_t)MR * cols, stream), "memset"); cuda_check(cudaMemsetAsync(sc, 0, (size_t)MR * 4, stream), "memset");
-            int r = make_tmap_u8_2d(tm, p, (uint64_t)MR, (uint64_t)cols, 128, 128);
-            if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for an fp8 activation buffer (code " + std::to_string(r) + ")");
-        };
-        q8(xn8_, sxn_, &tm_xn8_, H); q8(attn8_, sattn_, &tm_attn8_, qd); q8(act8_, sact_, &tm_act8_, F);
+    // projection inputs, zeroed (as their e4m3 copies): the GEMMs' stale rows stay finite
+    for (const auto& [a, cols] : {std::make_pair(&xn_, H), std::make_pair(&attn_, qd), std::make_pair(&act_, F)}) {
+        a->cols = cols;
+        a->x = dmalloc((size_t)MR * cols * 2);
+        cuda_check(cudaMemsetAsync(a->x, 0, (size_t)MR * cols * 2, stream), "memset");
+        amap(&a->tm, a->x, MR, cols);
+        if (!w8) continue;
+        a->q = reinterpret_cast<uint8_t*>(dmalloc((size_t)MR * cols)); a->sc = reinterpret_cast<float*>(dmalloc((size_t)MR * 4));
+        cuda_check(cudaMemsetAsync(a->q, 0, (size_t)MR * cols, stream), "memset"); cuda_check(cudaMemsetAsync(a->sc, 0, (size_t)MR * 4, stream), "memset");
+        tmap_check(make_tmap_u8_2d(&a->tm8, a->q, (uint64_t)MR, (uint64_t)cols, 128, 128), "an fp8 activation buffer");
     }
     cuda_check(cudaMemsetAsync(q_, 0, (size_t)MR * qd * 2, stream), "memset");
     // sampled rows (debug logits sample every row of a short prefill: up to 2048)
@@ -217,9 +213,8 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     cuda_check(cudaMemsetAsync(kv.base, 0, kv_pool_bytes, stream), "kv memset");   // stale pages must hold finite values (0*NaN; e4m3 0x00 = +0)
     {
         // fp8: the pool as rows of 128 bytes, one (page, kv head) block of K or V per box
-        int r = kv.fp8 ? make_tmap_u8_2d(&tm_kv, kv.base, (uint64_t)(kv_pool_bytes / 128), 128, (uint32_t)(D / 2), 128)
-                       : make_tmap_bf16_2d(&tm_kv, kv.base, (uint64_t)kv.layer_stride_rows * L, (uint64_t)D, (uint64_t)D, 64, 64);
-        if (r != 0) throw std::runtime_error("cuTensorMapEncodeTiled failed for the KV pool (code " + std::to_string(r) + ")");
+        tmap_check(kv.fp8 ? make_tmap_u8_2d(&tm_kv, kv.base, (uint64_t)(kv_pool_bytes / 128), 128, (uint32_t)(D / 2), 128)
+                          : make_tmap_bf16_2d(&tm_kv, kv.base, (uint64_t)kv.layer_stride_rows * L, (uint64_t)D, (uint64_t)D, 64, 64), "the KV pool");
     }
 
     // ---- decode-attention partial workspace + per-step metadata arena ----
@@ -261,183 +256,31 @@ DeviceModel::DeviceModel(const ModelConfig& c, const EngineOptions& o) : cfg(c),
     cuda_check(cudaStreamSynchronize(stream), "init sync");
 }
 
-// ---- Hugging Face checkpoint loading (Llama / Qwen2 naming) --------------------------------------------------------
-static float f16_bits_to_f32(uint16_t hb) {
-    const uint32_t h = hb, sign = (h & 0x8000u) << 16, e = (h >> 10) & 31, m = h & 1023; uint32_t f;
-    if (e == 0) { if (m == 0) f = sign; else { int sh = 0; uint32_t mm = m; while (!(mm & 1024)) { mm <<= 1; ++sh; } f = sign | ((uint32_t)(113 - sh) << 23) | ((mm & 1023) << 13); } }
-    else if (e == 31) f = sign | 0x7f800000u | (m << 13);
-    else f = sign | ((e + 112) << 23) | (m << 13);
-    float x; std::memcpy(&x, &f, 4); return x;
-}
-static void to_bf16_rows(const StTensor& t, int64_t C, int64_t row, int64_t col0, int64_t cols, uint16_t* dst) {
-    if (t.dtype == "BF16") { std::memcpy(dst, reinterpret_cast<const uint16_t*>(t.data) + row * C + col0, (size_t)cols * 2); return; }
-    if (t.dtype == "F32") { const float* s = reinterpret_cast<const float*>(t.data) + row * C + col0; for (int64_t i = 0; i < cols; ++i) dst[i] = f32_to_bf16_bits(s[i]); return; }
-    if (t.dtype == "F16") {
-        const uint16_t* s = reinterpret_cast<const uint16_t*>(t.data) + row * C + col0;
-        for (int64_t i = 0; i < cols; ++i) dst[i] = f32_to_bf16_bits(f16_bits_to_f32(s[i]));
-        return;
-    }
-    throw std::runtime_error("unsupported checkpoint dtype " + t.dtype);
-}
-
-// fp8 KV cache scales (compressed-tensors / vLLM naming): model.layers.{l}.self_attn.k_scale / v_scale, shape [] or [1], F32 / BF16 / F16,
-// finite and > 0, present for every layer or for none (then 1.0)
-static void load_kv_scales(const SafeTensors& st, int L, std::vector<float>& ks, std::vector<float>& vs) {
-    auto scalar = [&](const std::string& name) -> float {
-        const StTensor& t = st.get(name);
-        if (!(t.shape.empty() || (t.shape.size() == 1 && t.shape[0] == 1))) throw std::runtime_error("checkpoint tensor " + name + " must have shape [] or [1]");
-        float v;
-        if (t.dtype == "F32") std::memcpy(&v, t.data, 4);
-        else if (t.dtype == "BF16") { uint16_t b; std::memcpy(&b, t.data, 2); const uint32_t u = (uint32_t)b << 16; std::memcpy(&v, &u, 4); }
-        else if (t.dtype == "F16") { uint16_t b; std::memcpy(&b, t.data, 2); v = f16_bits_to_f32(b); }
-        else throw std::runtime_error("checkpoint tensor " + name + " has unsupported dtype " + t.dtype);
-        if (!std::isfinite(v) || v <= 0.f) throw std::runtime_error("checkpoint tensor " + name + " must be finite and > 0");
-        return v;
-    };
-    int nk = 0, nv = 0;
-    for (int l = 0; l < L; ++l) {
-        const std::string p = "model.layers." + std::to_string(l) + ".self_attn.";
-        nk += st.has(p + "k_scale"); nv += st.has(p + "v_scale");
-    }
-    if (nk == 0 && nv == 0) return;
-    for (const auto& c : {std::make_pair("k_scale", nk), std::make_pair("v_scale", nv)})
-        if (c.second != L) throw std::runtime_error("checkpoint has self_attn." + std::string(c.first) + " for " + std::to_string(c.second) + " of " +
-                                                    std::to_string(L) + " layers: KV cache scales must be given for every layer or for none");
-    for (int l = 0; l < L; ++l) {
-        const std::string p = "model.layers." + std::to_string(l) + ".self_attn.";
-        ks[l] = scalar(p + "k_scale"); vs[l] = scalar(p + "v_scale");
-    }
-}
-
+// ---- Hugging Face checkpoint loading (checkpoint.hpp assembles this rank's rows on the host) -------------------------------------------
 void DeviceModel::load_checkpoint(const std::string& path) {
-    // the seeded init (and, with fp8 weights, its quantisation through the scratch) is still queued on `stream`, which the synchronous copies
-    // below do not wait for
-    cuda_check(cudaStreamSynchronize(stream), "weight init");
     SafeTensors st(path);
-    const int H = cfg.hidden, L = cfg.n_layers, D = cfg.head_dim, V = cfg.vocab;
-    const int qd = nh_l * D, kd = nkv_l * D;
-    const int64_t r = tp_rank;
-    std::vector<uint16_t> buf;
-    // every tensor must have exactly the logical shape [R, C] (vectors: [C]) this model configuration implies — a transposed, truncated or
-    // wrong-config (hidden / ffn / heads / vocab) checkpoint is refused with a message instead of being read out of bounds
     const bool w8 = cfg.w_fp8();
-    auto checked = [&](const std::string& name, int64_t R, int64_t C) -> const StTensor& {
-        const StTensor& t = st.get(name);
-        const bool ok = (t.shape.size() == 2 && t.shape[0] == R && t.shape[1] == C) || (R == 1 && t.shape.size() == 1 && t.shape[0] == C);
-        if (!ok) {
-            std::string got = "["; for (size_t i = 0; i < t.shape.size(); ++i) got += (i ? ", " : "") + std::to_string(t.shape[i]); got += "]";
-            throw std::runtime_error("checkpoint tensor " + name + " has shape " + got + ", this model needs [" + (R == 1 ? "" : std::to_string(R) + ", ") + std::to_string(C) + "]");
-        }
-        const bool proj = name.size() > 12 && name.compare(name.size() - 12, 12, "_proj.weight") == 0;     // q/k/v/o/gate/up/down
-        if (proj && t.dtype == "F8_E4M3") {
-            if (!w8) throw std::runtime_error("checkpoint tensor " + name + " is F8_E4M3: fp8 projection weights need weight_dtype fp8_e4m3");
-            return t;
-        }
-        if (t.dtype != "BF16" && t.dtype != "F16" && t.dtype != "F32") throw std::runtime_error("checkpoint tensor " + name + " has unsupported dtype " + t.dtype);
-        return t;       // SafeTensors already verified bytes == prod(shape) * sizeof(dtype)
+    if (cfg.kv_fp8()) load_kv_scales(st, cfg.n_layers, kv_k_scale, kv_v_scale);
+    const CkptShard shard(st, cfg, tp, tp_rank);
+    std::vector<uint16_t> hb; std::vector<uint8_t> hq; std::vector<float> hs;
+    // every copy runs on `stream`, after the seeded init it overwrites, and lands before its host buffer is refilled: a pageable cudaMemcpy
+    // may return before its DMA lands, and it does not order with a non-blocking stream
+    auto h2d = [&](void* dst, const void* src, size_t bytes) { cuda_check(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream), "checkpoint H2D"); };
+    auto landed = [&]() { cuda_check(cudaStreamSynchronize(stream), "checkpoint H2D"); };
+    auto load = [&](const CkptRows& m, void* dst) { ckpt_bf16(st, m, hb); h2d(dst, hb.data(), hb.size() * 2); landed(); };
+    // a projection: bf16 / F16 / F32 parts through the same bf16 destination + commit as the seeded init; F8_E4M3 parts bring bytes and scales
+    auto load_proj = [&](WeightMat& w, const CkptRows& m) {
+        if (!ckpt_is_f8(st, m, w8)) { load(m, bf16_dst(w)); commit(w); return; }
+        ckpt_f8(st, m, hq, hs); h2d(w.ptr, hq.data(), hq.size()); h2d(w.sw, hs.data(), hs.size() * 4); landed();
     };
-    // logical [R, C] tensor `name`: rows [row0, row0+rows) x cols [col0, col0+cols) -> device dst (row-major [rows, cols])
-    auto slice = [&](const std::string& name, int64_t R, int64_t C, int64_t row0, int64_t rows, int64_t col0, int64_t cols, void* dst) {
-        const StTensor& t = checked(name, R, C);
-        if (row0 < 0 || col0 < 0 || row0 + rows > R || col0 + cols > C) throw std::runtime_error("checkpoint slice out of range for " + name);
-        buf.resize((size_t)rows * cols);
-        for (int64_t i = 0; i < rows; ++i) to_bf16_rows(t, C, row0 + i, col0, cols, buf.data() + (size_t)i * cols);
-        cuda_check(cudaMemcpy(dst, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
-    };
-    if (cfg.kv_fp8()) load_kv_scales(st, L, kv_k_scale, kv_v_scale);
-    // fp8 weights (tp == 1): projection w is assembled from whole checkpoint rows, rows[i] = (tensor name, its row count, source row) of
-    // physical row i.  bf16 / F16 / F32 parts are quantised on the device with the row rule; F8_E4M3 parts (compressed-tensors "FP8"
-    // checkpoints) bring their bytes and `<name>_scale` (per row [N, 1] / [N], or per tensor [] / [1]).  One matrix takes one kind.
-    // Static activation scales (`input_scale`) are not read: activations are quantised per token at run time.
-    struct SrcRow { const std::string* name; int64_t R, row; };
-    auto load_proj8 = [&](WeightMat& w, const std::vector<SrcRow>& rows) {
-        const int64_t K = w.K;
-        int n_f8 = 0;
-        for (const SrcRow& sr : rows) n_f8 += checked(*sr.name, sr.R, K).dtype == "F8_E4M3";
-        if (n_f8 == 0) {
-            std::vector<uint16_t> hb((size_t)w.N * K);
-            for (size_t i = 0; i < rows.size(); ++i) to_bf16_rows(st.get(*rows[i].name), K, rows[i].row, 0, K, hb.data() + i * K);
-            // on `stream`: a pageable cudaMemcpy may return before its DMA lands, and it does not order with a non-blocking stream
-            cuda_check(cudaMemcpyAsync(w8_scratch_, hb.data(), hb.size() * 2, cudaMemcpyHostToDevice, stream), "checkpoint H2D");
-            quantise_weight(w, w8_scratch_);
-            cuda_check(cudaStreamSynchronize(stream), "weight quantisation");
-            return;
-        }
-        if (n_f8 != (int)rows.size()) throw std::runtime_error("checkpoint tensor " + *rows[0].name + ": the parts of one fused projection (q/k/v, gate/up) must all be F8_E4M3 or none");
-        std::vector<uint8_t> hq((size_t)w.N * K); std::vector<float> hs((size_t)w.N);
-        std::map<std::string, std::vector<float>> scales;
-        for (size_t i = 0; i < rows.size(); ++i) {
-            const std::string& nm = *rows[i].name;
-            std::vector<float>& sc = scales[nm];
-            if (sc.empty()) {
-                const std::string sn = nm + "_scale";
-                if (!st.has(sn)) throw std::runtime_error("checkpoint tensor " + nm + " is F8_E4M3 but " + sn + " is missing");
-                const StTensor& t = st.get(sn);
-                const int64_t R = rows[i].R;
-                const bool per_row = (t.shape.size() == 2 && t.shape[0] == R && t.shape[1] == 1) || (t.shape.size() == 1 && t.shape[0] == R);
-                const bool per_tensor = t.shape.empty() || (t.shape.size() == 1 && t.shape[0] == 1) || (t.shape.size() == 2 && t.shape[0] == 1 && t.shape[1] == 1);
-                if (!per_row && !per_tensor) throw std::runtime_error("checkpoint tensor " + sn + " must have shape [" + std::to_string(R) + ", 1], [" + std::to_string(R) + "], [] or [1]");
-                const int64_t n = per_row ? R : 1;
-                sc.resize((size_t)R);
-                for (int64_t j = 0; j < n; ++j) {
-                    float v;
-                    if (t.dtype == "F32") std::memcpy(&v, t.data + 4 * j, 4);
-                    else if (t.dtype == "BF16") { uint16_t b; std::memcpy(&b, t.data + 2 * j, 2); const uint32_t u = (uint32_t)b << 16; std::memcpy(&v, &u, 4); }
-                    else if (t.dtype == "F16") { uint16_t b; std::memcpy(&b, t.data + 2 * j, 2); v = f16_bits_to_f32(b); }
-                    else throw std::runtime_error("checkpoint tensor " + sn + " has unsupported dtype " + t.dtype);
-                    if (!std::isfinite(v) || v <= 0.f) throw std::runtime_error("checkpoint tensor " + sn + " must be finite and > 0");
-                    sc[(size_t)j] = v;
-                }
-                if (!per_row) std::fill(sc.begin(), sc.end(), sc[0]);
-            }
-            std::memcpy(hq.data() + i * K, st.get(nm).data + (size_t)rows[i].row * K, (size_t)K);
-            hs[i] = sc[(size_t)rows[i].row];
-        }
-        cuda_check(cudaMemcpyAsync(w.ptr, hq.data(), hq.size(), cudaMemcpyHostToDevice, stream), "checkpoint H2D");
-        cuda_check(cudaMemcpyAsync(w.sw, hs.data(), hs.size() * 4, cudaMemcpyHostToDevice, stream), "checkpoint H2D");
-        cuda_check(cudaStreamSynchronize(stream), "checkpoint H2D");
-    };
-    slice("model.embed_tokens.weight", V, H, 0, V, 0, H, embed);
-    slice("model.norm.weight", 1, H, 0, 1, 0, H, final_norm);
-    if (!cfg.tie_embeddings) slice(st.has("lm_head.weight") ? "lm_head.weight" : "model.embed_tokens.weight", V, H, r * V_l, V_l, 0, H, lm_head.ptr);
-    for (int l = 0; l < L; ++l) {
-        Layer& ly = layers[l]; const std::string p = "model.layers." + std::to_string(l) + ".";
-        if (w8) {
-            const std::string nq = p + "self_attn.q_proj.weight", nk = p + "self_attn.k_proj.weight", nv = p + "self_attn.v_proj.weight";
-            const std::string no = p + "self_attn.o_proj.weight", ng = p + "mlp.gate_proj.weight", nu = p + "mlp.up_proj.weight", nd = p + "mlp.down_proj.weight";
-            std::vector<SrcRow> rq;
-            for (int64_t i = 0; i < qd; ++i) rq.push_back({&nq, qd, i});
-            for (int64_t i = 0; i < kd; ++i) rq.push_back({&nk, kd, i});
-            for (int64_t i = 0; i < kd; ++i) rq.push_back({&nv, kd, i});
-            load_proj8(ly.qkv, rq);
-            std::vector<SrcRow> ro, rg, rd;
-            for (int64_t i = 0; i < H; ++i) { ro.push_back({&no, H, i}); rd.push_back({&nd, H, i}); }
-            for (int64_t blk = 0; blk < F_l / 16; ++blk)
-                for (int64_t w = 0; w < 32; ++w) rg.push_back({w < 16 ? &ng : &nu, F_l, blk * 16 + (w & 15)});      // 16 gate rows, 16 up rows
-            load_proj8(ly.o, ro); load_proj8(ly.gu, rg); load_proj8(ly.down, rd);
-        } else {
-        uint16_t* wq = reinterpret_cast<uint16_t*>(ly.qkv.ptr);
-        slice(p + "self_attn.q_proj.weight", cfg.q_dim(), H, r * qd, qd, 0, H, wq);
-        slice(p + "self_attn.k_proj.weight", cfg.kv_dim(), H, r * kd, kd, 0, H, wq + (size_t)qd * H);
-        slice(p + "self_attn.v_proj.weight", cfg.kv_dim(), H, r * kd, kd, 0, H, wq + (size_t)(qd + kd) * H);
-        slice(p + "self_attn.o_proj.weight", H, cfg.q_dim(), 0, H, r * qd, qd, ly.o.ptr);
-        slice(p + "mlp.down_proj.weight", H, cfg.ffn, 0, H, r * F_l, F_l, ly.down.ptr);
-        // gate/up: physical rows interleaved in blocks of 16 (16 gate rows, 16 up rows)
-        const StTensor& tg = checked(p + "mlp.gate_proj.weight", cfg.ffn, H); const StTensor& tu = checked(p + "mlp.up_proj.weight", cfg.ffn, H);
-        buf.resize((size_t)2 * F_l * H);
-        for (int64_t blk = 0; blk < F_l / 16; ++blk)
-            for (int64_t w = 0; w < 32; ++w)
-                to_bf16_rows(w < 16 ? tg : tu, H, r * F_l + blk * 16 + (w & 15), 0, H, buf.data() + (size_t)(blk * 32 + w) * H);
-        cuda_check(cudaMemcpy(ly.gu.ptr, buf.data(), buf.size() * 2, cudaMemcpyHostToDevice), "checkpoint H2D");
-        }
-        slice(p + "input_layernorm.weight", 1, H, 0, 1, 0, H, ly.ln1);
-        slice(p + "post_attention_layernorm.weight", 1, H, 0, 1, 0, H, ly.ln2);
-        if (cfg.qkv_bias) {
-            uint16_t* bq = reinterpret_cast<uint16_t*>(ly.bqkv);
-            slice(p + "self_attn.q_proj.bias", 1, cfg.q_dim(), 0, 1, r * qd, qd, bq);
-            slice(p + "self_attn.k_proj.bias", 1, cfg.kv_dim(), 0, 1, r * kd, kd, bq + qd);
-            slice(p + "self_attn.v_proj.bias", 1, cfg.kv_dim(), 0, 1, r * kd, kd, bq + qd + kd);
-        }
+    load(shard.embed, embed);
+    load(shard.norm, final_norm);
+    if (!cfg.tie_embeddings) load(shard.lm_head, lm_head.ptr);
+    for (int l = 0; l < cfg.n_layers; ++l) {
+        Layer& ly = layers[l]; const CkptLayerRows& m = shard.layers[l];
+        load_proj(ly.qkv, m.qkv); load_proj(ly.o, m.o); load_proj(ly.gu, m.gu); load_proj(ly.down, m.down);
+        load(m.ln1, ly.ln1); load(m.ln2, ly.ln2);
+        if (cfg.qkv_bias) load(m.bqkv, ly.bqkv);
     }
 }
 
@@ -459,7 +302,7 @@ const char* DeviceModel::kt_name(int id) {
 }
 void DeviceModel::sync() { cuda_check(cudaStreamSynchronize(stream), "stream sync"); }
 void DeviceModel::sampled_logits(int S, float* out) {
-    const int n_tiles = gemm_n_tiles(cfg.vocab, pick_bn(S, cfg.vocab, opt.bn_lm, false));     // the LM head's per-tile row maxima of that forward
+    const int n_tiles = gemm_n_tiles(cfg.vocab, pick_bn(S, cfg.vocab, opt.bn_lm));     // the LM head's per-tile row maxima of that forward
     std::vector<float> v((size_t)S * n_tiles);
     cuda_check(cudaMemcpy(v.data(), amax_val_, v.size() * 4, cudaMemcpyDeviceToHost), "row maxima D2H");
     for (int r = 0; r < S; ++r) out[r] = *std::max_element(v.begin() + (size_t)r * n_tiles, v.begin() + (size_t)(r + 1) * n_tiles);
@@ -467,7 +310,7 @@ void DeviceModel::sampled_logits(int S, float* out) {
 
 // N-tile heuristic.  Decode (M <= 128) streams weights once: prefer the largest tile that still yields >= 1 CTA
 // per SM; prefill has M/128 row tiles as well, so the widest tile (least A re-reads) wins.
-int DeviceModel::pick_bn(int M, int N, int override_bn, bool swiglu) const {
+int DeviceModel::pick_bn(int M, int N, int override_bn) const {
     if (override_bn == 32 || override_bn == 64 || override_bn == 128 || override_bn == 256) return override_bn;
     const int m_tiles = (M + 127) / 128;
     // no 256-wide tile: its 64 x 256 fp32 fragment does not fit one consumer warpgroup's registers without spills
@@ -476,7 +319,6 @@ int DeviceModel::pick_bn(int M, int N, int override_bn, bool swiglu) const {
     // so wider tiles with fewer, longer-lived CTAs win as long as about half the SMs stream; many row tiles: fill every SM
     const long long want = m_tiles <= 2 ? sm_count / 2 : sm_count;
     for (int bn : cands) { if ((long long)((N + bn - 1) / bn) * m_tiles >= want) return bn; }
-    (void)swiglu;
     return 32;
 }
 
@@ -531,6 +373,15 @@ void build_decode_plan(const int32_t* ctx_lens, int n_seqs, int n_kv, int n_ctas
     }
     out.cta_ptr[(size_t)n_ctas] = (int32_t)k;
 }
+
+// cuda_check labels of the two row-parallel projections on the stream-K path and of the norm that follows each
+struct RowParallelLabels { const char *clusterk, *fused, *gemm, *norm, *resid, *nvls_part, *nvls_ar, *bf16_part, *f32_part, *ar; };
+static const RowParallelLabels kOLabels = {
+    "o gemm + residual (cluster split-K)", "o gemm + residual (stream-K)", "o gemm (stream-K)", "rmsnorm2", "resid+rmsnorm2", "o partial -> multicast buffer",
+    "in-switch allreduce+resid+rmsnorm2", "o partial -> symmetric buffer (bf16)", "o partial -> symmetric buffer", "allreduce+resid+rmsnorm2"};
+static const RowParallelLabels kDownLabels = {
+    "down gemm + residual (cluster split-K)", "down gemm + residual (stream-K)", "down gemm (stream-K)", "rmsnorm1", "resid+rmsnorm1", "down partial -> multicast buffer",
+    "in-switch allreduce+resid+rmsnorm1", "down partial -> symmetric buffer (bf16)", "down partial -> symmetric buffer", "allreduce+resid+rmsnorm1"};
 
 void DeviceModel::forward(const StepInput& in, float* logits_out) {
     const int T = (int)in.tokens.size(), S = (int)in.sample_rows.size();
@@ -601,23 +452,22 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
     cuda_check(launch_embed_gather(d_tok, embed, x_, T, H, cfg.vocab, stream), "embed"); MARK(0);
     // fp8 weights: every projection reads its input as e4m3 rows + per-row scales, quantised by one kernel right before the GEMM
     const bool w8 = cfg.w_fp8();
-    auto quant = [&](const void* x, uint8_t* q, float* sc, int C) { if (w8) { cuda_check(launch_quant_rows_e4m3(x, q, sc, T, C, stream), "fp8 quantise"); MARK(14); } };
-    const CUtensorMap *tA_xn = w8 ? &tm_xn8_ : &tm_xn_, *tA_attn = w8 ? &tm_attn8_ : &tm_attn_, *tA_act = w8 ? &tm_act8_ : &tm_act_;
-    auto w8s = [&](const float* sa, const WeightMat& w) { return w8 ? W8Scales{sa, w.sw} : W8Scales{}; };
+    auto quant = [&](const ProjInput& a) { if (a.q) { cuda_check(launch_quant_rows_e4m3(a.x, a.q, a.sc, T, a.cols, stream), "fp8 quantise"); MARK(14); } };
+    auto cap = [&](int bn) { return w8 ? std::min(bn, 128) : bn; };      // fp8 tiles are at most 128 wide (registers)
     // decode-sized batches (one or, opt-in, two 128-row tiles; fp8: one, the promoted fp8 fragment leaves no registers for a second)
     const bool use_sk = opt.streamk && T <= (w8 ? 128 : std::min(256, std::max(128, opt.sk_max_rows)));
     const int sk_rows = T > 128 ? 256 : 128;
     auto attention = [&](int l) {
         if (profile_attn) cudaEventRecord(ev[2 * l], stream);
         if (n_dec > 0) {
-            DecodeAttnParams a{}; a.q = q_; a.out = attn_; a.block_tables = d_bt; a.ctx_lens = d_ctx; a.max_pages_per_seq = max_pages_per_seq;
+            DecodeAttnParams a{}; a.q = q_; a.out = attn_.x; a.block_tables = d_bt; a.ctx_lens = d_ctx; a.max_pages_per_seq = max_pages_per_seq;
             a.segs = reinterpret_cast<const DecodeSeg*>(d_meta_ + o_segs); a.cta_seg_ptr = d_meta_ + o_ptr; a.n_ctas = (int)plan_.cta_ptr.size() - 1;
             a.part_o = part_o_; a.part_ml = part_ml_; a.layer = l; a.n_heads = nh; a.n_kv = nkv; a.scale_log2e = scale_log2e;
             a.merge_counters = d_meta_ + o_cnt;      // cut items are merged inside the kernel by the CTA finishing their last piece
             cuda_check(launch_decode_attention(&tm_kv, kv, a, stream), "decode attention"); MARK(4);
         }
         if (!in.decode && !in.tiles.empty()) {     // mixed step: both kernels, disjoint rows of q_/attn_
-            PrefillAttnParams a{}; a.q = q_; a.out = attn_; a.block_tables = d_bt; a.max_pages_per_seq = max_pages_per_seq;
+            PrefillAttnParams a{}; a.q = q_; a.out = attn_.x; a.block_tables = d_bt; a.max_pages_per_seq = max_pages_per_seq;
             a.tiles = reinterpret_cast<const PrefillTile*>(d_meta_ + o_tiles); a.n_tiles = (int)in.tiles.size();
             a.layer = l; a.n_heads = nh; a.n_kv = nkv; a.scale_log2e = scale_log2e;
             cuda_check(launch_prefill_attention(&tm_kv, kv, a, stream), "prefill attention");
@@ -627,14 +477,11 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
     };
     if (use_sk) {
         // decode-sized batch: persistent stream-K projections (fp32 partials) + fused consumers
-        auto bn_of = [&](int o) {      // two row tiles (and fp8) need BN <= 128 (registers)
-            const int bn = sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_);
-            return w8 ? std::min(bn, 128) : bn;
-        };
+        auto bn_of = [&](int o) { return cap(sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_)); };      // two row tiles need BN <= 128 (registers)
         auto with_pf = [&](StreamK k) { k.l2_prefetch_units = std::max(0, opt.sk_l2_prefetch_kb * 1024 / (k.bn * 128)); return k; };
         const StreamK sk_qkv = make_streamk(sk_ws_, qkvd, H, bn_of(opt.sk_bn_qkv), sk_G_, sk_rows, w8), sk_o = make_streamk(sk_ws_, H, qd, bn_of(opt.sk_bn_o), sk_G_, sk_rows, w8);
         const StreamK sk_gu = make_streamk(sk_ws_, 2 * F, H, bn_of(opt.sk_bn_gu), sk_G_, sk_rows, w8), sk_dn = make_streamk(sk_ws_, H, F, bn_of(opt.sk_bn_down), sk_G_, sk_rows, w8);
-        cuda_check(launch_rmsnorm(x_, layers[0].ln1, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
+        cuda_check(launch_rmsnorm(x_, layers[0].ln1, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
         const StreamK pf_qkv = with_pf(sk_qkv), pf_o = with_pf(sk_o), pf_gu = with_pf(sk_gu), pf_dn = with_pf(sk_dn);
         // qkv / o / down epilogues finished inside the GEMM (same conditions as the fused SwiGLU; every projection at BN = 128, tile counts within the flag arrays)
         const bool fuse_ok = sk_rows == 128 && sk_G_ <= sm_count && sk_qkv.bn == 128 && sk_o.bn == 128 && sk_dn.bn == 128 &&
@@ -646,92 +493,77 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         const int ck_o = (sk_rows == 128 && (opt.sk_clusterk & 2) && !use_tp) ? clusterk_pick(H, qd, sm_count, opt.sk_clusterk_min_fill) : 0;
         const int ck_dn = (sk_rows == 128 && (opt.sk_clusterk & 4) && !use_tp) ? clusterk_pick(H, F, sm_count, opt.sk_clusterk_min_fill) : 0;
         const bool fuse_swiglu = opt.sk_fuse_swiglu && !w8 && sk_rows == 128 && sk_gu.bn == 128 && sk_G_ <= sm_count && sk_gu.n_tiles <= SK_MAX_FLAG_TILES;
-        for (int l = 0; l < L; ++l) {
-            const Layer& ly = layers[l];
-            quant(xn_, xn8_, sxn_, H);
-            if (ck_qkv) {
-                cuda_check(launch_gemm_clusterk_rope(&tm_xn_, ly.qkv.map(128), T, qkvd, H, ck_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh), stream),
-                           "qkv gemm + RoPE + KV write (cluster split-K)"); MARK(2);
-            } else if (fuse_rope) {
-                cuda_check(launch_gemm_streamk_rope(tA_xn, ly.qkv.map(128), T, qkvd, H, pf_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh),
-                                                    tile_flags_ + 0 * SK_MAX_FLAG_TILES, stream, w8s(sxn_, ly.qkv)), "qkv gemm + RoPE + KV write (stream-K)"); MARK(2);
-            } else {
-                cuda_check(launch_gemm_streamk(tA_xn, ly.qkv.map(sk_qkv.bn), T, qkvd, H, pf_qkv, stream, w8s(sxn_, ly.qkv)), "qkv gemm (stream-K)"); MARK(2);
-                cuda_check(launch_sk_rope_kv_write(sk_qkv, ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope (stream-K)"); MARK(3);
+        // row-parallel projection (o, down): x += a . w^T, then xn = rmsnorm(x) * gain
+        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int K, int ck, bool fused, const StreamK& sk, const StreamK& pf, int flag_slot,
+                                const void* gain, int mark, const RowParallelLabels& lb) {
+            if (ck || fused) {
+                if (ck) cuda_check(launch_gemm_clusterk_resid(&a.tm, w.map(128), T, H, K, ck, x_, H, stream), lb.clusterk);
+                else cuda_check(launch_gemm_streamk_resid(a.map(), w.map(128), T, H, K, pf, x_, H, tile_flags_ + flag_slot * SK_MAX_FLAG_TILES, stream, a.w8(w)), lb.fused);
+                MARK(mark);
+                cuda_check(launch_rmsnorm_wide(x_, gain, xn_.x, T, H, cfg.rms_eps, stream), lb.norm); MARK(7);
+                return;
             }
-            attention(l);
-            quant(attn_, attn8_, sattn_, qd);
-            if (ck_o) {
-                cuda_check(launch_gemm_clusterk_resid(&tm_attn_, ly.o.map(128), T, H, qd, ck_o, x_, H, stream), "o gemm + residual (cluster split-K)"); MARK(6);
-                cuda_check(launch_rmsnorm_wide(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(7);
-            } else if (fuse_o) {
-                cuda_check(launch_gemm_streamk_resid(tA_attn, ly.o.map(128), T, H, qd, pf_o, x_, H, tile_flags_ + 1 * SK_MAX_FLAG_TILES, stream, w8s(sattn_, ly.o)), "o gemm + residual (stream-K)"); MARK(6);
-                cuda_check(launch_rmsnorm_wide(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(7);
-            } else {
-            cuda_check(launch_gemm_streamk(tA_attn, ly.o.map(sk_o.bn), T, H, qd, pf_o, stream, w8s(sattn_, ly.o)), "o gemm (stream-K)"); MARK(6);
+            cuda_check(launch_gemm_streamk(a.map(), w.map(sk.bn), T, H, K, pf, stream, a.w8(w)), lb.gemm); MARK(mark);
             if (use_tp) {      // row-parallel projection: all-reduce the rank partials over NVLink peer memory, then residual + norm
                 const int b = comm->next_buffer();
                 const TpComm::Signal sg = comm->next_signal();     // "buffer written" handshake rides on the two kernels: no barrier launch
                 if (comm->nvls() && T <= 128) {
                     char* loc = reinterpret_cast<char*>(comm->nvls_local());
-                    cuda_check(launch_sk_reduce_f32(sk_o, reinterpret_cast<float*>(loc + (size_t)b * nvls_region_), T, H, stream, &sg), "o partial -> multicast buffer");
+                    cuda_check(launch_sk_reduce_f32(sk, reinterpret_cast<float*>(loc + (size_t)b * nvls_region_), T, H, stream, &sg), lb.nvls_part);
                     cuda_check(launch_ar_nvls_resid_rmsnorm(comm->nvls_multicast(), loc, (size_t)b * nvls_region_, (size_t)(2 + b) * nvls_region_, 4 * nvls_region_ + (size_t)b * 512, tp, tp_rank,
-                                                            x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream, sg), "in-switch allreduce+resid+rmsnorm2");
+                                                            x_, gain, xn_.x, T, H, cfg.rms_eps, stream, sg), lb.nvls_ar);
                 } else if (opt.tp_ar_bf16) {
-                    cuda_check(launch_sk_reduce_bf16(sk_o, comm->sym(b), T, H, stream, &sg), "o partial -> symmetric buffer (bf16)");
-                    cuda_check(launch_ar_resid_rmsnorm_bf16in(comm->d_peer_sym(b), tp, x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream, &sg), "allreduce+resid+rmsnorm2");
+                    cuda_check(launch_sk_reduce_bf16(sk, comm->sym(b), T, H, stream, &sg), lb.bf16_part);
+                    cuda_check(launch_ar_resid_rmsnorm_bf16in(comm->d_peer_sym(b), tp, x_, gain, xn_.x, T, H, cfg.rms_eps, stream, &sg), lb.ar);
                 } else {
-                    cuda_check(launch_sk_reduce_f32(sk_o, reinterpret_cast<float*>(comm->sym(b)), T, H, stream, &sg), "o partial -> symmetric buffer");
-                    cuda_check(launch_ar_resid_rmsnorm(comm->d_peer_sym(b), tp, x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream, &sg), "allreduce+resid+rmsnorm2");
+                    cuda_check(launch_sk_reduce_f32(sk, reinterpret_cast<float*>(comm->sym(b)), T, H, stream, &sg), lb.f32_part);
+                    cuda_check(launch_ar_resid_rmsnorm(comm->d_peer_sym(b), tp, x_, gain, xn_.x, T, H, cfg.rms_eps, stream, &sg), lb.ar);
                 }
             } else {
-                cuda_check(launch_sk_resid_rmsnorm(sk_o, x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "resid+rmsnorm2");
+                cuda_check(launch_sk_resid_rmsnorm(sk, x_, gain, xn_.x, T, H, cfg.rms_eps, stream), lb.resid);
             }
             MARK(7);
+        };
+        for (int l = 0; l < L; ++l) {
+            const Layer& ly = layers[l];
+            quant(xn_);
+            if (ck_qkv) {
+                cuda_check(launch_gemm_clusterk_rope(&xn_.tm, ly.qkv.map(128), T, qkvd, H, ck_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh), stream),
+                           "qkv gemm + RoPE + KV write (cluster split-K)"); MARK(2);
+            } else if (fuse_rope) {
+                cuda_check(launch_gemm_streamk_rope(xn_.map(), ly.qkv.map(128), T, qkvd, H, pf_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh),
+                                                    tile_flags_ + 0 * SK_MAX_FLAG_TILES, stream, xn_.w8(ly.qkv)), "qkv gemm + RoPE + KV write (stream-K)"); MARK(2);
+            } else {
+                cuda_check(launch_gemm_streamk(xn_.map(), ly.qkv.map(sk_qkv.bn), T, qkvd, H, pf_qkv, stream, xn_.w8(ly.qkv)), "qkv gemm (stream-K)"); MARK(2);
+                cuda_check(launch_sk_rope_kv_write(sk_qkv, ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope (stream-K)"); MARK(3);
             }
-            quant(xn_, xn8_, sxn_, H);
+            attention(l);
+            quant(attn_);
+            row_parallel(attn_, ly.o, qd, ck_o, fuse_o, sk_o, pf_o, 1, ly.ln2, 6, kOLabels);
+            quant(xn_);
             if (fuse_swiglu) {
-                cuda_check(launch_gemm_streamk_swiglu(&tm_xn_, ly.gu.map(128), T, F, H, pf_gu, act_, tile_flags_ + 2 * SK_MAX_FLAG_TILES, stream), "gate_up gemm + SwiGLU (stream-K)"); MARK(8);
+                cuda_check(launch_gemm_streamk_swiglu(&xn_.tm, ly.gu.map(128), T, F, H, pf_gu, act_.x, tile_flags_ + 2 * SK_MAX_FLAG_TILES, stream), "gate_up gemm + SwiGLU (stream-K)"); MARK(8);
             } else {
-                cuda_check(launch_gemm_streamk(tA_xn, ly.gu.map(sk_gu.bn), T, 2 * F, H, pf_gu, stream, w8s(sxn_, ly.gu)), "gate_up gemm (stream-K)"); MARK(8);
-                cuda_check(launch_sk_swiglu(sk_gu, act_, T, F, stream), "swiglu"); MARK(9);
+                cuda_check(launch_gemm_streamk(xn_.map(), ly.gu.map(sk_gu.bn), T, 2 * F, H, pf_gu, stream, xn_.w8(ly.gu)), "gate_up gemm (stream-K)"); MARK(8);
+                cuda_check(launch_sk_swiglu(sk_gu, act_.x, T, F, stream), "swiglu"); MARK(9);
             }
-            quant(act_, act8_, sact_, F);
-            const void* next_gain = (l + 1 < L) ? layers[l + 1].ln1 : final_norm;
-            if (ck_dn) {
-                cuda_check(launch_gemm_clusterk_resid(&tm_act_, ly.down.map(128), T, H, F, ck_dn, x_, H, stream), "down gemm + residual (cluster split-K)"); MARK(10);
-                cuda_check(launch_rmsnorm_wide(x_, next_gain, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(7);
-                continue;
-            }
-            if (fuse_dn) {
-                cuda_check(launch_gemm_streamk_resid(tA_act, ly.down.map(128), T, H, F, pf_dn, x_, H, tile_flags_ + 3 * SK_MAX_FLAG_TILES, stream, w8s(sact_, ly.down)), "down gemm + residual (stream-K)"); MARK(10);
-                cuda_check(launch_rmsnorm_wide(x_, next_gain, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(7);
-                continue;
-            }
-            cuda_check(launch_gemm_streamk(tA_act, ly.down.map(sk_dn.bn), T, H, F, pf_dn, stream, w8s(sact_, ly.down)), "down gemm (stream-K)"); MARK(10);
-            if (use_tp) {
-                const int b = comm->next_buffer();
-                const TpComm::Signal sg = comm->next_signal();
-                if (comm->nvls() && T <= 128) {
-                    char* loc = reinterpret_cast<char*>(comm->nvls_local());
-                    cuda_check(launch_sk_reduce_f32(sk_dn, reinterpret_cast<float*>(loc + (size_t)b * nvls_region_), T, H, stream, &sg), "down partial -> multicast buffer");
-                    cuda_check(launch_ar_nvls_resid_rmsnorm(comm->nvls_multicast(), loc, (size_t)b * nvls_region_, (size_t)(2 + b) * nvls_region_, 4 * nvls_region_ + (size_t)b * 512, tp, tp_rank,
-                                                            x_, next_gain, xn_, T, H, cfg.rms_eps, stream, sg), "in-switch allreduce+resid+rmsnorm1");
-                } else if (opt.tp_ar_bf16) {
-                    cuda_check(launch_sk_reduce_bf16(sk_dn, comm->sym(b), T, H, stream, &sg), "down partial -> symmetric buffer (bf16)");
-                    cuda_check(launch_ar_resid_rmsnorm_bf16in(comm->d_peer_sym(b), tp, x_, next_gain, xn_, T, H, cfg.rms_eps, stream, &sg), "allreduce+resid+rmsnorm1");
-                } else {
-                    cuda_check(launch_sk_reduce_f32(sk_dn, reinterpret_cast<float*>(comm->sym(b)), T, H, stream, &sg), "down partial -> symmetric buffer");
-                    cuda_check(launch_ar_resid_rmsnorm(comm->d_peer_sym(b), tp, x_, next_gain, xn_, T, H, cfg.rms_eps, stream, &sg), "allreduce+resid+rmsnorm1");
-                }
-            } else {
-                cuda_check(launch_sk_resid_rmsnorm(sk_dn, x_, next_gain, xn_, T, H, cfg.rms_eps, stream), "resid+rmsnorm1");
-            }
-            MARK(7);
+            quant(act_);
+            row_parallel(act_, ly.down, F, ck_dn, fuse_dn, sk_dn, pf_dn, 3, (l + 1 < L) ? layers[l + 1].ln1 : final_norm, 10, kDownLabels);
         }
     } else {
-        // x += sum over ranks of the bf16 partials in symmetric buffer b (every rank's partial is complete: barrier passed)
-        auto allreduce_resid_bf16 = [&](int b) {
+        // row-parallel projection (o, down) into x.  Single GPU: the residual add in the epilogue.  Tensor parallel: bf16 partial -> symmetric
+        // buffer, barrier, x += sum over ranks (rank order)
+        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int K, int bn, int mark, const char* label) {
+            GemmParams g{}; g.M = T; g.N = H; g.K = K; g.ldo = H;
+            if (!use_tp) {
+                g.out = x_; g.resid = x_; g.ldr = H; g.w8 = a.w8(w);
+                cuda_check(launch_gemm(a.map(), w.map(bn), g, EPI_RESID, bn, stream), label); MARK(mark);
+                return;
+            }
+            const int b = comm->next_buffer();
+            g.out = comm->sym(b);
+            cuda_check(launch_gemm(&a.tm, w.map(bn), g, EPI_STORE, bn, stream), label); MARK(mark);
+            cuda_check(comm->barrier(stream), "xgpu barrier");
             if (T >= opt.tp_two_shot_rows) {
                 cuda_check(launch_ar2_reduce_scatter(comm->d_peer_sym(b), tp, tp_rank, x_, comm->sym(TpComm::GATHER), T, H, stream), "reduce-scatter+resid");
                 cuda_check(comm->barrier(stream), "xgpu barrier");
@@ -740,54 +572,35 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 cuda_check(launch_ar_resid_bf16(comm->d_peer_sym(b), tp, x_, T, H, stream), "allreduce+resid");
             }
         };
-        auto cap = [&](int bn) { return w8 ? std::min(bn, 128) : bn; };      // fp8 tiles are at most 128 wide (registers)
-        const int bn_qkv = cap(pick_bn(T, qkvd, opt.bn_qkv, false)), bn_o = cap(pick_bn(T, H, opt.bn_o, false));
-        const int bn_gu = cap(pick_bn(T, 2 * F, opt.bn_gu, true)), bn_down = cap(pick_bn(T, H, opt.bn_down, false));
+        const int bn_qkv = cap(pick_bn(T, qkvd, opt.bn_qkv)), bn_o = cap(pick_bn(T, H, opt.bn_o));
+        const int bn_gu = cap(pick_bn(T, 2 * F, opt.bn_gu)), bn_down = cap(pick_bn(T, H, opt.bn_down));
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
-            cuda_check(launch_rmsnorm(x_, ly.ln1, xn_, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
-            quant(xn_, xn8_, sxn_, H);
-            GemmParams g{}; g.M = T; g.N = qkvd; g.K = H; g.out = qkv_; g.ldo = qkvd; g.bias = ly.bqkv; g.w8 = w8s(sxn_, ly.qkv);
-            cuda_check(launch_gemm(tA_xn, ly.qkv.map(bn_qkv), g, EPI_STORE, bn_qkv, stream), "qkv gemm"); MARK(2);
+            cuda_check(launch_rmsnorm(x_, ly.ln1, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
+            quant(xn_);
+            GemmParams g{}; g.M = T; g.N = qkvd; g.K = H; g.out = qkv_; g.ldo = qkvd; g.bias = ly.bqkv; g.w8 = xn_.w8(ly.qkv);
+            cuda_check(launch_gemm(xn_.map(), ly.qkv.map(bn_qkv), g, EPI_STORE, bn_qkv, stream), "qkv gemm"); MARK(2);
             cuda_check(launch_rope_kv_write(qkv_, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope"); MARK(3);
             attention(l);
-            quant(attn_, attn8_, sattn_, qd);
-            if (use_tp) {      // bf16 partial -> symmetric buffer, barrier, x += sum over ranks (rank order)
-                const int b = comm->next_buffer();
-                GemmParams go{}; go.M = T; go.N = H; go.K = qd; go.out = comm->sym(b); go.ldo = H;
-                cuda_check(launch_gemm(&tm_attn_, ly.o.map(bn_o), go, EPI_STORE, bn_o, stream), "o gemm"); MARK(6);
-                cuda_check(comm->barrier(stream), "xgpu barrier");
-                allreduce_resid_bf16(b);
-            } else {
-                GemmParams go{}; go.M = T; go.N = H; go.K = qd; go.out = x_; go.ldo = H; go.resid = x_; go.ldr = H; go.w8 = w8s(sattn_, ly.o);
-                cuda_check(launch_gemm(tA_attn, ly.o.map(bn_o), go, EPI_RESID, bn_o, stream), "o gemm"); MARK(6);
-            }
-            cuda_check(launch_rmsnorm(x_, ly.ln2, xn_, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(1);
-            quant(xn_, xn8_, sxn_, H);
-            GemmParams gg{}; gg.M = T; gg.N = 2 * F; gg.K = H; gg.out = act_; gg.ldo = F; gg.w8 = w8s(sxn_, ly.gu);
-            cuda_check(launch_gemm(tA_xn, ly.gu.map(bn_gu), gg, EPI_SWIGLU, bn_gu, stream), "gate_up gemm"); MARK(8);
-            quant(act_, act8_, sact_, F);
-            if (use_tp) {
-                const int b = comm->next_buffer();
-                GemmParams gd{}; gd.M = T; gd.N = H; gd.K = F; gd.out = comm->sym(b); gd.ldo = H;
-                cuda_check(launch_gemm(&tm_act_, ly.down.map(bn_down), gd, EPI_STORE, bn_down, stream), "down gemm"); MARK(10);
-                cuda_check(comm->barrier(stream), "xgpu barrier");
-                allreduce_resid_bf16(b);
-            } else {
-                GemmParams gd{}; gd.M = T; gd.N = H; gd.K = F; gd.out = x_; gd.ldo = H; gd.resid = x_; gd.ldr = H; gd.w8 = w8s(sact_, ly.down);
-                cuda_check(launch_gemm(tA_act, ly.down.map(bn_down), gd, EPI_RESID, bn_down, stream), "down gemm"); MARK(10);
-            }
+            quant(attn_);
+            row_parallel(attn_, ly.o, qd, bn_o, 6, "o gemm");
+            cuda_check(launch_rmsnorm(x_, ly.ln2, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(1);
+            quant(xn_);
+            GemmParams gg{}; gg.M = T; gg.N = 2 * F; gg.K = H; gg.out = act_.x; gg.ldo = F; gg.w8 = xn_.w8(ly.gu);
+            cuda_check(launch_gemm(xn_.map(), ly.gu.map(bn_gu), gg, EPI_SWIGLU, bn_gu, stream), "gate_up gemm"); MARK(8);
+            quant(act_);
+            row_parallel(act_, ly.down, F, bn_down, 10, "down gemm");
         }
     }
     if (S > 0) {
         if (use_sk) {      // xn_ already holds final_norm(x): just pick the sampled rows
-            cuda_check(launch_gather_rows(xn_, d_samp, xsn_, S, H, stream), "gather");
+            cuda_check(launch_gather_rows(xn_.x, d_samp, xsn_, S, H, stream), "gather");
         } else {
             cuda_check(launch_gather_rows(x_, d_samp, xs_, S, H, stream), "gather");
             cuda_check(launch_rmsnorm(xs_, final_norm, xsn_, S, H, cfg.rms_eps, stream), "final norm");
         }
         MARK(11);
-        const int bn_lm = pick_bn(S, V, opt.bn_lm, false);
+        const int bn_lm = pick_bn(S, V, opt.bn_lm);
         const int n_tiles = gemm_n_tiles(V, bn_lm);
         GemmParams gl{}; gl.M = S; gl.N = V; gl.K = H; gl.logits = logits_out; gl.ldl = V; gl.amax_val = amax_val_; gl.amax_idx = amax_idx_;
         if (!in.mask_slots.empty()) {          // constrained rows: the arg-max runs over their state's allowed tokens, on every vocabulary shard

@@ -18,6 +18,15 @@ struct WeightMat {
     const CUtensorMap* map(int bn) const { return &tm[bn == 32 ? 0 : bn == 64 ? 1 : bn == 128 ? 2 : 3]; }
 };
 
+// A projection's input: the bf16 activation buffer [max rows, cols] and, with fp8 weights, its e4m3 copy with one fp32 scale per row,
+// which the GEMMs read instead (quantised right before each projection)
+struct ProjInput {
+    void* x = nullptr; CUtensorMap tm; int cols = 0;
+    uint8_t* q = nullptr; float* sc = nullptr; CUtensorMap tm8;      // fp8 weights only
+    const CUtensorMap* map() const { return q ? &tm8 : &tm; }
+    W8Scales w8(const WeightMat& w) const { return q ? W8Scales{sc, w.sw} : W8Scales{}; }
+};
+
 struct StepInput {
     bool decode = false;
     int n_decode = 0;                                 // mixed step (decode == false): the first n_decode rows / sequences are decoding sequences
@@ -78,18 +87,19 @@ public:
 
 private:
     void alloc_weight(WeightMat& w, int N, int K, bool fp8 = false);
-    void quantise_weight(WeightMat& w, const void* bf16);      // fp8: bf16 [N, K] on the device -> w's bytes and row scales (row rule)
+    // a projection weight is written as bf16 [N, K] to bf16_dst(w) (fp8: the shared scratch), then commit(w) quantises an fp8 one into its
+    // bytes and row scales (row rule)
+    uint16_t* bf16_dst(const WeightMat& w) const { return reinterpret_cast<uint16_t*>(w.fp8 ? w8_scratch_ : w.ptr); }
+    void commit(WeightMat& w);
     void load_checkpoint(const std::string& path);     // overwrite the seeded tensors with this rank's slices of an HF checkpoint
     void make_weight_maps(WeightMat& w);
-    int pick_bn(int M, int N, int override_bn, bool swiglu) const;
+    int pick_bn(int M, int N, int override_bn) const;
     void* dmalloc(size_t bytes);
     std::vector<void*> allocs_;
     // activations
-    void *x_ = nullptr, *xn_ = nullptr, *qkv_ = nullptr, *q_ = nullptr, *attn_ = nullptr, *act_ = nullptr, *xs_ = nullptr, *xsn_ = nullptr;
-    CUtensorMap tm_xn_, tm_attn_, tm_act_, tm_xsn_;
-    // fp8 weights: the projection inputs quantised per row (e4m3 bytes + fp32 scales), allocated only then
-    uint8_t *xn8_ = nullptr, *attn8_ = nullptr, *act8_ = nullptr; float *sxn_ = nullptr, *sattn_ = nullptr, *sact_ = nullptr;
-    CUtensorMap tm_xn8_, tm_attn8_, tm_act8_;
+    void *x_ = nullptr, *qkv_ = nullptr, *q_ = nullptr, *xs_ = nullptr, *xsn_ = nullptr;
+    ProjInput xn_, attn_, act_;                    // inputs of qkv and gate/up, of o, of down
+    CUtensorMap tm_xsn_;
     void* w8_scratch_ = nullptr;                   // bf16 staging of one projection while the weights are generated or loaded (then freed)
     float* amax_val_ = nullptr; int* amax_idx_ = nullptr; int32_t* d_out_ids_ = nullptr;
     uint32_t* mask_table_ = nullptr;               // [mask_slots][mask_words] allowed-token bitsets of grammar states (filled on demand by the scheduler)
