@@ -167,6 +167,36 @@ OA_API int oa_k_gemm_fp8(const void* A, const float* sa, const void* B, const fl
  * fuse 2 = x [M, N] bf16 += product, finished inside the GEMM */
 OA_API int oa_k_gemm_streamk_fp8(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t block_n,
                                  int32_t n_ctas, int32_t fuse, void* x, float* out_f32, void* stream);
+/* The decode step's finished projections, launched as DeviceModel::forward launches them (test entry points, not the serving path).  A [M, K]
+ * and B [N, K] are bf16, or e4m3 bytes with fp32 row scales sa [M] / sb [N] (null for bf16).  path 0 = stream-K GEMM (block_n 64 / 128 / 256,
+ * two 128-row slots when M > 128) + the stand-alone consumer; 1 = stream-K GEMM with the finisher fused (block_n 128); 2 / 3 / 4 / 8 = cluster
+ * split-K with that cluster size (bf16).  Each call owns its stream-K workspace and zeroed tile flags.  A launcher's refusal returns
+ * OA_ERR_BAD_REQUEST, any other CUDA error OA_ERR_INTERNAL. */
+/* o / down: x [M, N] bf16 += A.B^T, then xn = rmsnorm(x) * gain; `launches` repeats both back to back on the same tile flags */
+OA_API int oa_k_sk_row_parallel(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t block_n,
+                                int32_t n_ctas, int32_t path, void* x, const void* gain, void* xn, float eps, int32_t launches, void* stream);
+/* gate/up: act [M, F] = silu(gate) * up from B [2F, K] (16 gate rows, then 16 up rows per 32); paths 0 and 1 (bf16 only) */
+OA_API int oa_k_sk_swiglu(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t F, int32_t K, int32_t block_n,
+                          int32_t n_ctas, int32_t path, void* act, int32_t launches, void* stream);
+/* qkv: (+ bias) -> bf16 -> RoPE -> q_out and one layer of a paged cache laid out as for oa_k_paged_attention (k_scale <= 0: bf16) or
+ * oa_k_paged_attention_fp8; positions / slots [M] on the device */
+OA_API int oa_k_sk_qkv_rope(const void* A, const float* sa, const void* B, const float* sb, const void* bias, int32_t M, int32_t K, int32_t n_heads,
+                            int32_t n_kv, int32_t head_dim, int32_t block_n, int32_t n_ctas, int32_t path, const int32_t* positions, const int32_t* slots,
+                            const float* rope_cos, const float* rope_sin, void* q_out, void* kv_cache, int32_t num_pages, float k_scale, float v_scale,
+                            void* stream);
+/* oa_k_kv_write_fp8 on a bf16 cache (the prefill writer) */
+OA_API int oa_k_kv_write(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos, const float* rope_sin, void* q_out,
+                         void* kv_cache, int32_t num_pages, int32_t T, int32_t n_heads, int32_t n_kv, int32_t head_dim, void* stream);
+/* decode attention on the engine's work plan for n_ctas_target CTAs (host block_tables / ctx_lens as oa_k_paged_attention).  merge_inline:
+ * cut items are merged inside the kernel on merge counters zeroed once, `launches` times in a row; else by the separate merge kernel.
+ * k_scale <= 0: bf16 cache */
+OA_API int oa_k_decode_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
+                                 int32_t max_pages_per_seq, const int32_t* ctx_lens, int32_t n_seqs, int32_t n_heads, int32_t n_kv, int32_t head_dim,
+                                 int32_t n_ctas_target, int32_t merge_inline, int32_t launches, float k_scale, float v_scale, void* stream);
+/* the LM head: fp32 logits [M, N] and ids [M] = the arg-max of each row (ties: lowest id).  A row r with mask_slot[r] >= 0 takes it over the
+ * ids whose bit (col_offset + column) is set in mask_table[mask_slot[r] * mask_words ...], 0 when none is (all device pointers) */
+OA_API int oa_k_gemm_logits_masked(const void* A, const void* B, int32_t M, int32_t N, int32_t K, int32_t block_n, const uint32_t* mask_table,
+                                   const int32_t* mask_slot, int32_t mask_words, int32_t col_offset, float* logits, int32_t* ids, void* stream);
 /* ---- host-only logic, callable without a GPU (CPU tests) ---- */
 /* chat template + tokenizer of the model described by config_json */
 OA_API int oa_host_apply_chat_template(const char* config_json, const oa_msg* msgs, int32_t n_msgs, int32_t* out_ids, int32_t cap, int32_t* n_out);

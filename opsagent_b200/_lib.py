@@ -37,6 +37,7 @@ SYMBOLS = [
     "oa_k_gemm_streamk", "oa_debug_kernel_times", "oa_engine_serve", "oa_host_grammar_step", "oa_host_grammar_step_ex", "oa_host_grammar_token_mask", "oa_http_start", "oa_http_port", "oa_http_stats", "oa_http_stop", "oa_http_last_error", "oa_host_json_roundtrip", "oa_chat_cancel", "oa_chat_submit_ex", "oa_chat_wait_ex",
     "oa_k_paged_attention_fp8", "oa_k_kv_write_fp8",
     "oa_k_quant_rows_e4m3", "oa_k_gemm_fp8", "oa_k_gemm_streamk_fp8",
+    "oa_k_sk_row_parallel", "oa_k_sk_swiglu", "oa_k_sk_qkv_rope", "oa_k_kv_write", "oa_k_decode_attention", "oa_k_gemm_logits_masked",
 ]
 
 _lib = None
@@ -80,6 +81,14 @@ def load() -> C.CDLL:
     L.oa_k_quant_rows_e4m3.argtypes = [vp, vp, vp, i32, i32, vp]; L.oa_k_quant_rows_e4m3.restype = C.c_int
     L.oa_k_gemm_fp8.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp]; L.oa_k_gemm_fp8.restype = C.c_int
     L.oa_k_gemm_streamk_fp8.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]; L.oa_k_gemm_streamk_fp8.restype = C.c_int
+    L.oa_k_sk_row_parallel.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, f32, i32, vp]; L.oa_k_sk_row_parallel.restype = C.c_int
+    L.oa_k_sk_swiglu.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, i32, vp]; L.oa_k_sk_swiglu.restype = C.c_int
+    L.oa_k_sk_qkv_rope.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, f32, f32, vp]
+    L.oa_k_sk_qkv_rope.restype = C.c_int
+    L.oa_k_kv_write.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]; L.oa_k_kv_write.restype = C.c_int
+    L.oa_k_decode_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, f32, vp]
+    L.oa_k_decode_attention.restype = C.c_int
+    L.oa_k_gemm_logits_masked.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp, vp]; L.oa_k_gemm_logits_masked.restype = C.c_int
     L.oa_host_apply_chat_template.argtypes = [C.c_char_p, C.POINTER(OaMsg), i32, vp, i32, C.POINTER(i32)]; L.oa_host_apply_chat_template.restype = C.c_int
     L.oa_host_bpe_encode.argtypes = [C.c_char_p, C.c_char_p, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_encode.restype = C.c_int
     L.oa_host_bpe_decode.argtypes = [C.c_char_p, vp, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_decode.restype = C.c_int

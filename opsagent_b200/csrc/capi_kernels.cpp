@@ -28,6 +28,27 @@ struct DevBuf {
     ~DevBuf() { if (p) cudaFree(p); }
 };
 int rc_of(cudaError_t e) { return e == cudaSuccess ? OA_OK : OA_ERR_INTERNAL; }
+// the same, telling a launcher's refusal of its arguments apart from a failed launch
+int rc_launch(cudaError_t e) { return e == cudaErrorInvalidValue ? OA_ERR_BAD_REQUEST : rc_of(e); }
+
+// A [M, K] and B [N, K] operand maps of a decode projection as the engine builds them: bf16 (boxes {64, 128} / {64, bn}) or, with row
+// scales, e4m3 bytes (boxes {128, 128} / {128, bn})
+bool proj_maps(CUtensorMap* tmA, CUtensorMap* tmB, const void* A, const void* B, bool fp8, int M, int N, int K, int bn) {
+    if (fp8) return make_tmap_u8_2d(tmA, A, (uint64_t)M, (uint64_t)K, 128, 128) == 0 && make_tmap_u8_2d(tmB, B, (uint64_t)N, (uint64_t)K, (uint32_t)bn, 128) == 0;
+    return make_tmap_bf16_2d(tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)K, 128, 64) == 0 &&
+           make_tmap_bf16_2d(tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)bn, 64) == 0;
+}
+// one projection's stream-K workspace and zeroed per-tile flags (the engine's sk_ws_ / tile_flags_)
+struct SkSetup {
+    DevBuf ws, flags; StreamK sk;
+    SkSetup(int N, int K, int bn, int G, int rows, bool fp8, cudaStream_t s)
+        : ws(streamk_ws_bytes(N, bn, G, rows)), flags((size_t)SK_MAX_FLAG_TILES * 4), sk(make_streamk((float*)ws.p, N, K, bn, G, rows, fp8)) {
+        if (flags.p && cudaMemsetAsync(flags.p, 0, (size_t)SK_MAX_FLAG_TILES * 4, s) != cudaSuccess) { cudaFree(flags.p); flags.p = nullptr; }
+    }
+    bool ok() const { return ws.p && flags.p; }
+    unsigned int* tile_flags() const { return (unsigned int*)flags.p; }
+};
+bool is_cluster_path(int path) { return path >= 2; }
 
 // one layer of a paged cache: bf16, or fp8 with the given scales (k_scale / v_scale point at one float each)
 KvLayout one_layer_kv(const void* kv_cache, int32_t num_pages, int32_t n_kv, int32_t head_dim, const float* k_scale, const float* v_scale) {
@@ -43,6 +64,8 @@ int kv_tmap(CUtensorMap* tm, const KvLayout& kv) {
 
 int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
                     const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s);
+int decode_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                     int32_t n_seqs, int32_t n_heads, int32_t n_ctas_target, int32_t force_splits, bool merge_inline, int32_t launches, cudaStream_t s);
 }  // namespace
 
 // test-only: materialise the deterministic fixed-order sum of stream-K partials as fp32 [M,N]
@@ -131,17 +154,24 @@ int oa_k_gemm(const void* A, const void* B, int32_t M, int32_t N, int32_t K, int
     if (make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)block_n, 64) != 0) return OA_ERR_INTERNAL;
     GemmParams p{}; p.M = M; p.N = N; p.K = K; p.out = out; p.ldo = epilogue == EPI_SWIGLU ? N / 2 : N;
     p.bias = bias; p.resid = resid; p.ldr = N; p.logits = logits; p.ldl = N;
-    if (epilogue == EPI_LOGITS) {
-        const int nt = gemm_n_tiles(N, block_n);
-        DevBuf av((size_t)M * nt * 4), ai((size_t)M * nt * 4);
-        if (!av.p || !ai.p) return OA_ERR_INTERNAL;
-        p.amax_val = (float*)av.p; p.amax_idx = (int*)ai.p;
-        cudaError_t e = launch_gemm(&tmA, &tmB, p, epilogue, block_n, s);
-        if (e == cudaSuccess) e = launch_argmax_reduce(p.amax_val, p.amax_idx, M, nt, argmax_out, nullptr, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        return rc_of(e);
-    }
+    if (epilogue == EPI_LOGITS) return oa_k_gemm_logits_masked(A, B, M, N, K, block_n, nullptr, nullptr, 0, 0, logits, argmax_out, stream);
     return rc_of(launch_gemm(&tmA, &tmB, p, epilogue, block_n, s));
+}
+
+int oa_k_gemm_logits_masked(const void* A, const void* B, int32_t M, int32_t N, int32_t K, int32_t block_n, const uint32_t* mask_table,
+                            const int32_t* mask_slot, int32_t mask_words, int32_t col_offset, float* logits, int32_t* ids, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    CUtensorMap tmA, tmB;
+    if (!proj_maps(&tmA, &tmB, A, B, false, M, N, K, block_n)) return OA_ERR_INTERNAL;
+    const int nt = gemm_n_tiles(N, block_n);
+    DevBuf av((size_t)M * nt * 4), ai((size_t)M * nt * 4);
+    if (!av.p || !ai.p) return OA_ERR_INTERNAL;
+    GemmParams p{}; p.M = M; p.N = N; p.K = K; p.logits = logits; p.ldl = N; p.amax_val = (float*)av.p; p.amax_idx = (int*)ai.p;
+    p.mask_table = mask_table; p.mask_slot = mask_slot; p.mask_words = mask_words; p.col_offset = col_offset;
+    cudaError_t e = launch_gemm(&tmA, &tmB, p, EPI_LOGITS, block_n, s);
+    if (e == cudaSuccess) e = launch_argmax_reduce(p.amax_val, p.amax_idx, M, nt, ids, nullptr, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
 }
 
 int oa_k_paged_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
@@ -168,41 +198,118 @@ int oa_k_kv_write_fp8(const void* qkv, const int32_t* positions, const int32_t* 
     return rc_of(e);
 }
 
+int oa_k_kv_write(const void* qkv, const int32_t* positions, const int32_t* slots, const float* rope_cos, const float* rope_sin, void* q_out,
+                  void* kv_cache, int32_t num_pages, int32_t T, int32_t n_heads, int32_t n_kv, int32_t head_dim, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const KvLayout kv = one_layer_kv(kv_cache, num_pages, n_kv, head_dim, nullptr, nullptr);
+    cudaError_t e = launch_rope_kv_write(qkv, positions, slots, rope_cos, rope_sin, q_out, kv, 0, T, n_heads, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_sk_row_parallel(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t N, int32_t K, int32_t block_n,
+                         int32_t n_ctas, int32_t path, void* x, const void* gain, void* xn, float eps, int32_t launches, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool fp8 = sa != nullptr, ck = is_cluster_path(path);
+    if (path < 0 || (ck && fp8)) return OA_ERR_BAD_REQUEST;
+    const int bn = path == 0 ? block_n : 128;
+    CUtensorMap tmA, tmB;
+    if (!proj_maps(&tmA, &tmB, A, B, fp8, M, N, K, bn)) return OA_ERR_INTERNAL;
+    SkSetup st(N, K, bn, n_ctas, path == 0 && M > 128 ? 256 : 128, fp8, s);
+    if (!st.ok()) return OA_ERR_INTERNAL;
+    const W8Scales w8{sa, sb};
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < launches && e == cudaSuccess; ++i) {
+        if (path == 0) {
+            e = launch_gemm_streamk(&tmA, &tmB, M, N, K, st.sk, s, w8);
+            if (e == cudaSuccess) e = launch_sk_resid_rmsnorm(st.sk, x, gain, xn, M, N, eps, s);
+            continue;
+        }
+        e = ck ? launch_gemm_clusterk_resid(&tmA, &tmB, M, N, K, path, x, N, s)
+               : launch_gemm_streamk_resid(&tmA, &tmB, M, N, K, st.sk, x, N, st.tile_flags(), s, w8);
+        if (e == cudaSuccess) e = launch_rmsnorm_wide(x, gain, xn, M, N, eps, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_sk_swiglu(const void* A, const float* sa, const void* B, const float* sb, int32_t M, int32_t F, int32_t K, int32_t block_n,
+                   int32_t n_ctas, int32_t path, void* act, int32_t launches, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool fp8 = sa != nullptr;
+    if (path != 0 && path != 1) return OA_ERR_BAD_REQUEST;
+    const int bn = path == 0 ? block_n : 128;
+    CUtensorMap tmA, tmB;
+    if (!proj_maps(&tmA, &tmB, A, B, fp8, M, 2 * F, K, bn)) return OA_ERR_INTERNAL;
+    SkSetup st(2 * F, K, bn, n_ctas, path == 0 && M > 128 ? 256 : 128, fp8, s);
+    if (!st.ok()) return OA_ERR_INTERNAL;
+    const W8Scales w8{sa, sb};
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < launches && e == cudaSuccess; ++i) {
+        if (path == 0) {
+            e = launch_gemm_streamk(&tmA, &tmB, M, 2 * F, K, st.sk, s, w8);
+            if (e == cudaSuccess) e = launch_sk_swiglu(st.sk, act, M, F, s);
+        } else {
+            e = launch_gemm_streamk_swiglu(&tmA, &tmB, M, F, K, st.sk, act, st.tile_flags(), s, w8);
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_sk_qkv_rope(const void* A, const float* sa, const void* B, const float* sb, const void* bias, int32_t M, int32_t K, int32_t n_heads,
+                     int32_t n_kv, int32_t head_dim, int32_t block_n, int32_t n_ctas, int32_t path, const int32_t* positions, const int32_t* slots,
+                     const float* rope_cos, const float* rope_sin, void* q_out, void* kv_cache, int32_t num_pages, float k_scale, float v_scale,
+                     void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool fp8 = sa != nullptr, ck = is_cluster_path(path);
+    if (path < 0 || (ck && fp8)) return OA_ERR_BAD_REQUEST;
+    const int N = (n_heads + 2 * n_kv) * head_dim, bn = path == 0 ? block_n : 128;
+    CUtensorMap tmA, tmB;
+    if (!proj_maps(&tmA, &tmB, A, B, fp8, M, N, K, bn)) return OA_ERR_INTERNAL;
+    SkSetup st(N, K, bn, n_ctas, path == 0 && M > 128 ? 256 : 128, fp8, s);
+    if (!st.ok()) return OA_ERR_INTERNAL;
+    const bool kv8 = k_scale > 0.f;
+    const KvLayout kv = one_layer_kv(kv_cache, num_pages, n_kv, head_dim, kv8 ? &k_scale : nullptr, kv8 ? &v_scale : nullptr);
+    const SkRopeArgs rope = make_sk_rope_args(bias, positions, slots, rope_cos, rope_sin, q_out, kv, 0, n_heads);
+    cudaError_t e;
+    if (path == 0) {
+        e = launch_gemm_streamk(&tmA, &tmB, M, N, K, st.sk, s, W8Scales{sa, sb});
+        if (e == cudaSuccess) e = launch_sk_rope_kv_write(st.sk, bias, positions, slots, rope_cos, rope_sin, q_out, kv, 0, M, n_heads, s);
+    } else if (ck) {
+        e = launch_gemm_clusterk_rope(&tmA, &tmB, M, N, K, path, rope, s);
+    } else {
+        e = launch_gemm_streamk_rope(&tmA, &tmB, M, N, K, st.sk, rope, st.tile_flags(), s, W8Scales{sa, sb});
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_decode_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables, int32_t max_pages_per_seq,
+                          const int32_t* ctx_lens, int32_t n_seqs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t n_ctas_target,
+                          int32_t merge_inline, int32_t launches, float k_scale, float v_scale, void* stream) {
+    const bool kv8 = k_scale > 0.f;
+    return decode_attention(q, out, one_layer_kv(kv_cache, num_pages, n_kv, head_dim, kv8 ? &k_scale : nullptr, kv8 ? &v_scale : nullptr), block_tables,
+                            max_pages_per_seq, ctx_lens, n_seqs, n_heads, n_ctas_target, 0, merge_inline != 0, launches, (cudaStream_t)stream);
+}
+
 }  // extern "C"
 
 namespace {
 int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
                     const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s) {
     const int n_kv = kv.n_kv, head_dim = kv.head_dim;
+    bool decode = true;
+    for (int i = 0; i < n_seqs; ++i) if (q_lens && q_lens[i] != 1) decode = false;
+    if (decode) return decode_attention(q, out, kv, block_tables, max_pages_per_seq, ctx_lens, n_seqs, n_heads, 2 * 132, force_splits, false, 1, s);
     CUtensorMap tm;
     if (kv_tmap(&tm, kv) != 0) return OA_ERR_INTERNAL;
     const float scale_log2e = (1.0f / std::sqrt((float)head_dim)) * 1.4426950408889634f;
-    const int grp = n_heads / n_kv;
-    bool decode = true; int total_q = 0;
-    for (int i = 0; i < n_seqs; ++i) { if (q_lens && q_lens[i] != 1) decode = false; total_q += q_lens ? q_lens[i] : 1; }
     DevBuf d_bt((size_t)n_seqs * max_pages_per_seq * 4), d_ctx((size_t)n_seqs * 4);
     if (!d_bt.p || !d_ctx.p) return OA_ERR_INTERNAL;
     cudaMemcpyAsync(d_bt.p, block_tables, (size_t)n_seqs * max_pages_per_seq * 4, cudaMemcpyHostToDevice, s);
     cudaMemcpyAsync(d_ctx.p, ctx_lens, (size_t)n_seqs * 4, cudaMemcpyHostToDevice, s);
     cudaError_t e;
-    if (decode) {
-        DecodePlan plan;
-        build_decode_plan(ctx_lens, n_seqs, n_kv, 2 * 132, force_splits, plan);
-        DevBuf d_segs(plan.segs.size() * sizeof(DecodeSeg)), d_ptr(plan.cta_ptr.size() * 4), d_merge(plan.merges.size() * sizeof(MergeItem));
-        DevBuf d_po((size_t)(plan.n_slots + 1) * grp * head_dim * 4), d_pml((size_t)(plan.n_slots + 1) * grp * 2 * 4);
-        if (!d_segs.p || !d_ptr.p || !d_merge.p || !d_po.p || !d_pml.p) return OA_ERR_INTERNAL;
-        cudaMemcpyAsync(d_segs.p, plan.segs.data(), plan.segs.size() * sizeof(DecodeSeg), cudaMemcpyHostToDevice, s);
-        cudaMemcpyAsync(d_ptr.p, plan.cta_ptr.data(), plan.cta_ptr.size() * 4, cudaMemcpyHostToDevice, s);
-        cudaMemcpyAsync(d_merge.p, plan.merges.data(), plan.merges.size() * sizeof(MergeItem), cudaMemcpyHostToDevice, s);
-        DecodeAttnParams a{}; a.q = q; a.out = out; a.block_tables = (const int32_t*)d_bt.p; a.ctx_lens = (const int32_t*)d_ctx.p;
-        a.max_pages_per_seq = max_pages_per_seq; a.segs = (const DecodeSeg*)d_segs.p; a.cta_seg_ptr = (const int32_t*)d_ptr.p;
-        a.n_ctas = (int)plan.cta_ptr.size() - 1; a.part_o = (float*)d_po.p; a.part_ml = (float*)d_pml.p; a.layer = 0;
-        a.n_heads = n_heads; a.n_kv = n_kv; a.scale_log2e = scale_log2e;
-        e = launch_decode_attention(&tm, kv, a, s);
-        if (e == cudaSuccess) e = launch_decode_merge((const MergeItem*)d_merge.p, (int)plan.merges.size(), a.part_o, a.part_ml, out, n_heads, n_kv, head_dim, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        return rc_of(e);
-    }
     std::vector<PrefillTile> tiles; int row = 0;
     for (int i = 0; i < n_seqs; ++i) {
         const int ql = q_lens[i], p0 = ctx_lens[i] - ql;
@@ -217,6 +324,40 @@ int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t*
     e = launch_prefill_attention(&tm, kv, a, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     return rc_of(e);
+}
+
+// one decode-attention step on build_decode_plan's work plan.  merge_inline: the engine's in-kernel merge, on counters zeroed once and carried
+// across `launches` launches (they advance by n_pieces per launch, as per layer in a step); else the separate merge kernel after each launch
+int decode_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                     int32_t n_seqs, int32_t n_heads, int32_t n_ctas_target, int32_t force_splits, bool merge_inline, int32_t launches, cudaStream_t s) {
+    const int n_kv = kv.n_kv, head_dim = kv.head_dim, grp = n_heads / n_kv;
+    CUtensorMap tm;
+    if (kv_tmap(&tm, kv) != 0) return OA_ERR_INTERNAL;
+    DecodePlan plan;
+    build_decode_plan(ctx_lens, n_seqs, n_kv, n_ctas_target, force_splits, plan);
+    DevBuf d_bt((size_t)n_seqs * max_pages_per_seq * 4), d_ctx((size_t)n_seqs * 4);
+    DevBuf d_segs(plan.segs.size() * sizeof(DecodeSeg)), d_ptr(plan.cta_ptr.size() * 4), d_merge(plan.merges.size() * sizeof(MergeItem));
+    DevBuf d_po((size_t)(plan.n_slots + 1) * grp * head_dim * 4), d_pml((size_t)(plan.n_slots + 1) * grp * 2 * 4), d_cnt((plan.merges.size() + 1) * 4);
+    if (!d_bt.p || !d_ctx.p || !d_segs.p || !d_ptr.p || !d_merge.p || !d_po.p || !d_pml.p || !d_cnt.p) return OA_ERR_INTERNAL;
+    cudaMemcpyAsync(d_bt.p, block_tables, (size_t)n_seqs * max_pages_per_seq * 4, cudaMemcpyHostToDevice, s);
+    cudaMemcpyAsync(d_ctx.p, ctx_lens, (size_t)n_seqs * 4, cudaMemcpyHostToDevice, s);
+    cudaMemcpyAsync(d_segs.p, plan.segs.data(), plan.segs.size() * sizeof(DecodeSeg), cudaMemcpyHostToDevice, s);
+    cudaMemcpyAsync(d_ptr.p, plan.cta_ptr.data(), plan.cta_ptr.size() * 4, cudaMemcpyHostToDevice, s);
+    cudaMemcpyAsync(d_merge.p, plan.merges.data(), plan.merges.size() * sizeof(MergeItem), cudaMemcpyHostToDevice, s);
+    cudaMemsetAsync(d_cnt.p, 0, (plan.merges.size() + 1) * 4, s);
+    DecodeAttnParams a{}; a.q = q; a.out = out; a.block_tables = (const int32_t*)d_bt.p; a.ctx_lens = (const int32_t*)d_ctx.p;
+    a.max_pages_per_seq = max_pages_per_seq; a.segs = (const DecodeSeg*)d_segs.p; a.cta_seg_ptr = (const int32_t*)d_ptr.p;
+    a.n_ctas = (int)plan.cta_ptr.size() - 1; a.part_o = (float*)d_po.p; a.part_ml = (float*)d_pml.p; a.layer = 0;
+    a.merge_counters = merge_inline ? (int32_t*)d_cnt.p : nullptr;
+    a.n_heads = n_heads; a.n_kv = n_kv; a.scale_log2e = (1.0f / std::sqrt((float)head_dim)) * 1.4426950408889634f;
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < launches && e == cudaSuccess; ++i) {
+        e = launch_decode_attention(&tm, kv, a, s);
+        if (e == cudaSuccess && !merge_inline)
+            e = launch_decode_merge((const MergeItem*)d_merge.p, (int)plan.merges.size(), a.part_o, a.part_ml, out, n_heads, n_kv, head_dim, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
 }
 }  // namespace
 

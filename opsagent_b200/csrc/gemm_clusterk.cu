@@ -58,7 +58,7 @@ __global__ void OA_GEMM_REGS gemm_clusterk_kernel(const __grid_constant__ CUtens
     const uint32_t rank = ck_cluster_rank();
     const int tile = (int)blockIdx.x / S;
     const int kb_total = (K + BLOCK_K - 1) / BLOCK_K;
-    const int kb0 = (int)((long long)rank * kb_total / S), kb1 = (int)((long long)(rank + 1) * kb_total / S), n_kb = kb1 - kb0;   // host: kb_total >= S
+    const int kb0 = (int)((long long)rank * kb_total / S), kb1 = (int)((long long)(rank + 1) * kb_total / S), n_kb = kb1 - kb0;   // kb_total >= S (the launchers refuse less)
 
     float d[1][CK_BN / 2] = {};
     if (warp == PRODUCER_WARP) {
@@ -168,13 +168,16 @@ int clusterk_pick(int N, int K, int sms, int min_fill_pct) {
     return 0;
 }
 
+// every CTA of a cluster must own at least one k-block (the kernel's kb_total >= S)
+static bool ck_too_short(int K, int S) { return (K + BLOCK_K - 1) / BLOCK_K < S; }
+
 cudaError_t launch_gemm_clusterk_resid(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, int S, void* x, int ldx, cudaStream_t stream) {
-    if (M <= 0 || M > BLOCK_M || (N % 8) != 0 || (K % 8) != 0 || !x || (ldx % 8) != 0) return cudaErrorInvalidValue;
+    if (M <= 0 || M > BLOCK_M || (N % 8) != 0 || (K % 8) != 0 || !x || (ldx % 8) != 0 || ck_too_short(K, S)) return cudaErrorInvalidValue;
     CkEpi ep{}; ep.kind = 2; ep.x = reinterpret_cast<uint16_t*>(x); ep.ldx = ldx; ep.N = N;
     return launch_ck_s<128>(S, tmA, tmB, M, N, K, ep, stream);          // D only fixes the unit pairing: any pairing suits the residual epilogue
 }
 cudaError_t launch_gemm_clusterk_rope(const CUtensorMap* tmA, const CUtensorMap* tmB, int M, int N, int K, int S, const SkRopeArgs& rope, cudaStream_t stream) {
-    if (M <= 0 || M > BLOCK_M || (K % 8) != 0 || N != (rope.nh + 2 * rope.nkv) * rope.D) return cudaErrorInvalidValue;
+    if (M <= 0 || M > BLOCK_M || (K % 8) != 0 || N != (rope.nh + 2 * rope.nkv) * rope.D || ck_too_short(K, S)) return cudaErrorInvalidValue;
     CkEpi ep{}; ep.kind = 3; ep.N = N; ep.rope = rope;
     if (rope.D == 128) return launch_ck_s<128>(S, tmA, tmB, M, N, K, ep, stream);
     if (rope.D == 64) return launch_ck_s<64>(S, tmA, tmB, M, N, K, ep, stream);
