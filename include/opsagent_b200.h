@@ -197,7 +197,27 @@ OA_API int oa_k_decode_attention(const void* q, void* out, const void* kv_cache,
  * ids whose bit (col_offset + column) is set in mask_table[mask_slot[r] * mask_words ...], 0 when none is (all device pointers) */
 OA_API int oa_k_gemm_logits_masked(const void* A, const void* B, int32_t M, int32_t N, int32_t K, int32_t block_n, const uint32_t* mask_table,
                                    const int32_t* mask_slot, int32_t mask_words, int32_t col_offset, float* logits, int32_t* ids, void* stream);
+/* The prefill step's tile-path kernels, launched as DeviceModel::forward launches them (test entry points, synchronous, each allocating what it
+ * needs; a launcher's refusal returns OA_ERR_BAD_REQUEST).
+ * Projection GEMM: A [a_rows, K] (a_rows >= M: the map spans a_rows rows, as the engine's activation maps span max_step_tokens) and B [N, K],
+ * bf16, or e4m3 bytes with fp32 row scales sa / sb (null for bf16).  epilogue 0: out [M, N] = A.B^T (+ bias [N]); 1: out [M, N] += A.B^T in
+ * place; 2: out [M, N/2] = silu(gate) * up (B rows 16 gate / 16 up per 32).  block_n 0 = the engine's choice (pick_bn, fp8 capped at 128);
+ * the BLOCK_N used goes to *block_n_used.  The persistent or the tile kernel runs as launch_gemm decides (OA_GEMM_PERSISTENT /
+ * OA_GEMM_PERSISTENT_MIN_TILES). */
+OA_API int oa_k_prefill_gemm(const void* A, const float* sa, const void* B, const float* sb, int32_t a_rows, int32_t M, int32_t N, int32_t K,
+                             int32_t epilogue, int32_t block_n, void* out, const void* bias, int32_t* block_n_used, void* stream);
+/* One layer's attention of a prefill or mixed step on one paged cache (laid out as for oa_k_paged_attention, or oa_k_paged_attention_fp8 when
+ * k_scale > 0).  Sequences 0 .. n_decode-1 have one query row each (rows 0 .. n_decode-1) and run decode attention on the engine's plan for
+ * 2 x SMs CTAs with the in-kernel merge; the others have q_lens[i] rows each, the last at position ctx_lens[i] - 1, and run as the engine's
+ * 128-row prefill tiles, heaviest first.  Both kernels on one stream, decode first.  block_tables / ctx_lens / q_lens on the host. */
+OA_API int oa_k_step_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables,
+                               int32_t max_pages_per_seq, const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs, int32_t n_decode,
+                               int32_t n_heads, int32_t n_kv, int32_t head_dim, float k_scale, float v_scale, void* stream);
+/* out [T, H] = table [vocab, H] rows of ids [T] (device); an id outside [0, vocab) reads row 0 */
+OA_API int oa_k_embed_gather(const int32_t* ids, const void* table, void* out, int32_t T, int32_t H, int32_t vocab, void* stream);
 /* ---- host-only logic, callable without a GPU (CPU tests) ---- */
+/* BLOCK_N of the engine's tile-path GEMM [M, N] on sm_count SMs (pick_bn; override_bn in {32, 64, 128, 256} wins, fp8 != 0 caps it at 128) */
+OA_API int32_t oa_host_pick_bn(int32_t M, int32_t N, int32_t sm_count, int32_t override_bn, int32_t fp8);
 /* chat template + tokenizer of the model described by config_json */
 OA_API int oa_host_apply_chat_template(const char* config_json, const oa_msg* msgs, int32_t n_msgs, int32_t* out_ids, int32_t cap, int32_t* n_out);
 /* decode-attention work plan: segs_out[cap_segs*5] = {seq, kvh, chunk_begin, chunk_end, partial_slot}, cta_ptr_out[n_ctas+1];

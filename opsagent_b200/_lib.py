@@ -38,6 +38,7 @@ SYMBOLS = [
     "oa_k_paged_attention_fp8", "oa_k_kv_write_fp8",
     "oa_k_quant_rows_e4m3", "oa_k_gemm_fp8", "oa_k_gemm_streamk_fp8",
     "oa_k_sk_row_parallel", "oa_k_sk_swiglu", "oa_k_sk_qkv_rope", "oa_k_kv_write", "oa_k_decode_attention", "oa_k_gemm_logits_masked",
+    "oa_k_prefill_gemm", "oa_k_step_attention", "oa_k_embed_gather", "oa_host_pick_bn",
 ]
 
 _lib = None
@@ -89,6 +90,10 @@ def load() -> C.CDLL:
     L.oa_k_decode_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, f32, vp]
     L.oa_k_decode_attention.restype = C.c_int
     L.oa_k_gemm_logits_masked.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp, vp]; L.oa_k_gemm_logits_masked.restype = C.c_int
+    L.oa_k_prefill_gemm.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, C.POINTER(i32), vp]; L.oa_k_prefill_gemm.restype = C.c_int
+    L.oa_k_step_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, f32, f32, vp]; L.oa_k_step_attention.restype = C.c_int
+    L.oa_k_embed_gather.argtypes = [vp, vp, vp, i32, i32, i32, vp]; L.oa_k_embed_gather.restype = C.c_int
+    L.oa_host_pick_bn.argtypes = [i32, i32, i32, i32, i32]; L.oa_host_pick_bn.restype = i32
     L.oa_host_apply_chat_template.argtypes = [C.c_char_p, C.POINTER(OaMsg), i32, vp, i32, C.POINTER(i32)]; L.oa_host_apply_chat_template.restype = C.c_int
     L.oa_host_bpe_encode.argtypes = [C.c_char_p, C.c_char_p, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_encode.restype = C.c_int
     L.oa_host_bpe_decode.argtypes = [C.c_char_p, vp, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_decode.restype = C.c_int

@@ -66,6 +66,9 @@ int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t*
                     const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s);
 int decode_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
                      int32_t n_seqs, int32_t n_heads, int32_t n_ctas_target, int32_t force_splits, bool merge_inline, int32_t launches, cudaStream_t s);
+int prefill_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                      const int32_t* q_lens, int32_t seq0, int32_t n_seqs, int32_t n_heads, cudaStream_t s);
+int sm_count() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n > 0 ? n : 132; }
 }  // namespace
 
 // test-only: materialise the deterministic fixed-order sum of stream-K partials as fp32 [M,N]
@@ -285,6 +288,47 @@ int oa_k_sk_qkv_rope(const void* A, const float* sa, const void* B, const float*
     return rc_launch(e);
 }
 
+int oa_k_prefill_gemm(const void* A, const float* sa, const void* B, const float* sb, int32_t a_rows, int32_t M, int32_t N, int32_t K, int32_t epilogue,
+                      int32_t block_n, void* out, const void* bias, int32_t* block_n_used, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool fp8 = sa != nullptr;
+    if (a_rows < M || epilogue < EPI_STORE || epilogue > EPI_SWIGLU) return OA_ERR_BAD_REQUEST;
+    const int bn = block_n ? block_n : pick_bn(M, N, sm_count(), 0, fp8);
+    if (block_n_used) *block_n_used = bn;
+    CUtensorMap tmA, tmB;
+    if (!proj_maps(&tmA, &tmB, A, B, fp8, a_rows, N, K, bn)) return OA_ERR_INTERNAL;
+    GemmParams p{}; p.M = M; p.N = N; p.K = K; p.out = out; p.ldo = epilogue == EPI_SWIGLU ? N / 2 : N;
+    if (epilogue == EPI_STORE) p.bias = bias;
+    if (epilogue == EPI_RESID) { p.resid = out; p.ldr = N; }
+    p.w8 = W8Scales{sa, sb};
+    cudaError_t e = launch_gemm(&tmA, &tmB, p, epilogue, bn, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_step_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables, int32_t max_pages_per_seq,
+                        const int32_t* ctx_lens, const int32_t* q_lens, int32_t n_seqs, int32_t n_decode, int32_t n_heads, int32_t n_kv,
+                        int32_t head_dim, float k_scale, float v_scale, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n_decode < 0 || n_decode > n_seqs) return OA_ERR_BAD_REQUEST;
+    for (int i = 0; i < n_seqs; ++i) if (q_lens[i] < 1 || q_lens[i] > ctx_lens[i] || (i < n_decode && q_lens[i] != 1)) return OA_ERR_BAD_REQUEST;
+    const bool kv8 = k_scale > 0.f;
+    const KvLayout kv = one_layer_kv(kv_cache, num_pages, n_kv, head_dim, kv8 ? &k_scale : nullptr, kv8 ? &v_scale : nullptr);
+    if (n_decode > 0) {
+        const int rc = decode_attention(q, out, kv, block_tables, max_pages_per_seq, ctx_lens, n_decode, n_heads, 2 * sm_count(), 0, true, 1, s);
+        if (rc != OA_OK) return rc;
+    }
+    if (n_decode == n_seqs) return OA_OK;
+    return prefill_attention(q, out, kv, block_tables, max_pages_per_seq, ctx_lens, q_lens, n_decode, n_seqs, n_heads, s);
+}
+
+int oa_k_embed_gather(const int32_t* ids, const void* table, void* out, int32_t T, int32_t H, int32_t vocab, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    cudaError_t e = launch_embed_gather(ids, table, out, T, H, vocab, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
 int oa_k_decode_attention(const void* q, void* out, const void* kv_cache, int32_t num_pages, const int32_t* block_tables, int32_t max_pages_per_seq,
                           const int32_t* ctx_lens, int32_t n_seqs, int32_t n_heads, int32_t n_kv, int32_t head_dim, int32_t n_ctas_target,
                           int32_t merge_inline, int32_t launches, float k_scale, float v_scale, void* stream) {
@@ -298,32 +342,36 @@ int oa_k_decode_attention(const void* q, void* out, const void* kv_cache, int32_
 namespace {
 int paged_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
                     const int32_t* q_lens, int32_t n_seqs, int32_t n_heads, int32_t force_splits, cudaStream_t s) {
-    const int n_kv = kv.n_kv, head_dim = kv.head_dim;
     bool decode = true;
     for (int i = 0; i < n_seqs; ++i) if (q_lens && q_lens[i] != 1) decode = false;
     if (decode) return decode_attention(q, out, kv, block_tables, max_pages_per_seq, ctx_lens, n_seqs, n_heads, 2 * 132, force_splits, false, 1, s);
+    const int rc = prefill_attention(q, out, kv, block_tables, max_pages_per_seq, ctx_lens, q_lens, 0, n_seqs, n_heads, s);
+    return rc == OA_ERR_BAD_REQUEST ? OA_ERR_INTERNAL : rc;
+}
+
+// prefill attention of sequences seq0 .. n_seqs-1 (q_lens[i] new rows each, after the sum of q_lens[0 .. seq0-1] rows of the token batch):
+// their 128-row tiles, built and ordered as the engine's prefill step builds and orders them
+int prefill_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
+                      const int32_t* q_lens, int32_t seq0, int32_t n_seqs, int32_t n_heads, cudaStream_t s) {
     CUtensorMap tm;
     if (kv_tmap(&tm, kv) != 0) return OA_ERR_INTERNAL;
-    const float scale_log2e = (1.0f / std::sqrt((float)head_dim)) * 1.4426950408889634f;
-    DevBuf d_bt((size_t)n_seqs * max_pages_per_seq * 4), d_ctx((size_t)n_seqs * 4);
-    if (!d_bt.p || !d_ctx.p) return OA_ERR_INTERNAL;
-    cudaMemcpyAsync(d_bt.p, block_tables, (size_t)n_seqs * max_pages_per_seq * 4, cudaMemcpyHostToDevice, s);
-    cudaMemcpyAsync(d_ctx.p, ctx_lens, (size_t)n_seqs * 4, cudaMemcpyHostToDevice, s);
-    cudaError_t e;
+    const float scale_log2e = (1.0f / std::sqrt((float)kv.head_dim)) * 1.4426950408889634f;
     std::vector<PrefillTile> tiles; int row = 0;
-    for (int i = 0; i < n_seqs; ++i) {
-        const int ql = q_lens[i], p0 = ctx_lens[i] - ql;
-        for (int r = 0; r < ql; r += PREFILL_TILE_ROWS) tiles.push_back(PrefillTile{i, row + r, p0 + r, std::min(PREFILL_TILE_ROWS, ql - r)});
-        row += ql;
+    for (int i = 0; i < seq0; ++i) row += q_lens[i];
+    for (int i = seq0; i < n_seqs; ++i) {
+        append_prefill_tiles(tiles, i, row, ctx_lens[i] - q_lens[i], q_lens[i]);
+        row += q_lens[i];
     }
-    DevBuf d_tiles(tiles.size() * sizeof(PrefillTile));
-    if (!d_tiles.p) return OA_ERR_INTERNAL;
+    sort_prefill_tiles(tiles);
+    DevBuf d_bt((size_t)n_seqs * max_pages_per_seq * 4), d_tiles(tiles.size() * sizeof(PrefillTile));
+    if (!d_bt.p || !d_tiles.p) return OA_ERR_INTERNAL;
+    cudaMemcpyAsync(d_bt.p, block_tables, (size_t)n_seqs * max_pages_per_seq * 4, cudaMemcpyHostToDevice, s);
     cudaMemcpyAsync(d_tiles.p, tiles.data(), tiles.size() * sizeof(PrefillTile), cudaMemcpyHostToDevice, s);
     PrefillAttnParams a{}; a.q = q; a.out = out; a.block_tables = (const int32_t*)d_bt.p; a.max_pages_per_seq = max_pages_per_seq;
-    a.tiles = (const PrefillTile*)d_tiles.p; a.n_tiles = (int)tiles.size(); a.layer = 0; a.n_heads = n_heads; a.n_kv = n_kv; a.scale_log2e = scale_log2e;
-    e = launch_prefill_attention(&tm, kv, a, s);
+    a.tiles = (const PrefillTile*)d_tiles.p; a.n_tiles = (int)tiles.size(); a.layer = 0; a.n_heads = n_heads; a.n_kv = kv.n_kv; a.scale_log2e = scale_log2e;
+    cudaError_t e = launch_prefill_attention(&tm, kv, a, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    return rc_of(e);
+    return rc_launch(e);
 }
 
 // one decode-attention step on build_decode_plan's work plan.  merge_inline: the engine's in-kernel merge, on counters zeroed once and carried
@@ -406,6 +454,10 @@ int oa_host_streamk_plan(int32_t N, int32_t K, int32_t block_n, int32_t n_ctas, 
     }
     *n_ctas_out = sk.G; *n_tiles_out = sk.n_tiles; *kb_out = sk.kb;
     return OA_OK;
+}
+
+int32_t oa_host_pick_bn(int32_t M, int32_t N, int32_t sm_count, int32_t override_bn, int32_t fp8) {
+    return pick_bn(M, N, sm_count, override_bn, fp8 != 0);
 }
 
 int oa_host_grammar_step(int32_t kind, const uint8_t* prefix, int32_t n, uint32_t* mask_out, int32_t* done_out) {

@@ -172,7 +172,7 @@ public:
             for (size_t i = 0; i < pages.size(); ++i) in.block_tables[i] = pages[i];
             in.ctx_lens = {n};
             for (int i = 0; i < n; ++i) { in.tokens.push_back(toks[i]); in.positions.push_back(i); in.slots.push_back(pages[i / 64] * 64 + i % 64); in.sample_rows.push_back(i); }
-            for (int r = 0; r < n; r += PREFILL_TILE_ROWS) in.tiles.push_back(PrefillTile{0, r, r, std::min(PREFILL_TILE_ROWS, n - r)});
+            append_prefill_tiles(in.tiles, 0, 0, 0, n);
             run_forward(in, d_logits); model_.sync();
             cudaError_t e = cudaMemcpy(logits_out, d_logits, (size_t)n * V * 4, cudaMemcpyDeviceToHost);
             cudaFree(d_logits);
@@ -218,7 +218,7 @@ public:
                         in.ctx_lens.push_back(off + take);
                         const int row0 = (int)in.tokens.size();
                         for (int i = off; i < off + take; ++i) { in.tokens.push_back(synth(b, i)); in.positions.push_back(i); in.slots.push_back(pages[b][i / 64] * 64 + i % 64); }
-                        for (int r = 0; r < take; r += PREFILL_TILE_ROWS) in.tiles.push_back(PrefillTile{sidx, row0 + r, off + r, std::min(PREFILL_TILE_ROWS, take - r)});
+                        append_prefill_tiles(in.tiles, sidx, row0, off, take);
                         budget -= take; off += take;
                         if (off >= P) { off = 0; ++b; }
                     }
@@ -574,7 +574,7 @@ private:
                     for (int i = s->n_cached; i < s->n_cached + take; ++i) {
                         in.tokens.push_back(s->tokens[i]); in.positions.push_back(i); in.slots.push_back(s->pages[i / 64] * 64 + i % 64);
                     }
-                    for (int r = 0; r < take; r += PREFILL_TILE_ROWS) in.tiles.push_back(PrefillTile{sidx, row0 + r, s->n_cached + r, std::min(PREFILL_TILE_ROWS, take - r)});
+                    append_prefill_tiles(in.tiles, sidx, row0, s->n_cached, take);
                     if (take == remaining) { in.sample_rows.push_back(row0 + take - 1); sampled.push_back(s); }
                     batch.push_back(s); take_of.push_back(take); budget -= take;
                 }

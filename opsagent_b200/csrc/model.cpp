@@ -302,7 +302,7 @@ const char* DeviceModel::kt_name(int id) {
 }
 void DeviceModel::sync() { cuda_check(cudaStreamSynchronize(stream), "stream sync"); }
 void DeviceModel::sampled_logits(int S, float* out) {
-    const int n_tiles = gemm_n_tiles(cfg.vocab, pick_bn(S, cfg.vocab, opt.bn_lm));     // the LM head's per-tile row maxima of that forward
+    const int n_tiles = gemm_n_tiles(cfg.vocab, pick_bn(S, cfg.vocab, sm_count, opt.bn_lm));     // the LM head's per-tile row maxima of that forward
     std::vector<float> v((size_t)S * n_tiles);
     cuda_check(cudaMemcpy(v.data(), amax_val_, v.size() * 4, cudaMemcpyDeviceToHost), "row maxima D2H");
     for (int r = 0; r < S; ++r) out[r] = *std::max_element(v.begin() + (size_t)r * n_tiles, v.begin() + (size_t)(r + 1) * n_tiles);
@@ -310,7 +310,8 @@ void DeviceModel::sampled_logits(int S, float* out) {
 
 // N-tile heuristic.  Decode (M <= 128) streams weights once: prefer the largest tile that still yields >= 1 CTA
 // per SM; prefill has M/128 row tiles as well, so the widest tile (least A re-reads) wins.
-int DeviceModel::pick_bn(int M, int N, int override_bn) const {
+int pick_bn(int M, int N, int sm_count, int override_bn, bool fp8) {
+    if (fp8) return std::min(pick_bn(M, N, sm_count, override_bn), W8_MAX_BN);
     if (override_bn == 32 || override_bn == 64 || override_bn == 128 || override_bn == 256) return override_bn;
     const int m_tiles = (M + 127) / 128;
     // no 256-wide tile: its 64 x 256 fp32 fragment does not fit one consumer warpgroup's registers without spills
@@ -320,6 +321,15 @@ int DeviceModel::pick_bn(int M, int N, int override_bn) const {
     const long long want = m_tiles <= 2 ? sm_count / 2 : sm_count;
     for (int bn : cands) { if ((long long)((N + bn - 1) / bn) * m_tiles >= want) return bn; }
     return 32;
+}
+
+void append_prefill_tiles(std::vector<PrefillTile>& tiles, int seq, int row0, int pos0, int n_rows) {
+    for (int r = 0; r < n_rows; r += PREFILL_TILE_ROWS) tiles.push_back(PrefillTile{seq, row0 + r, pos0 + r, std::min(PREFILL_TILE_ROWS, n_rows - r)});
+}
+
+void sort_prefill_tiles(std::vector<PrefillTile>& tiles) {
+    // the causal triangle otherwise leaves a long tail of big CTAs
+    std::stable_sort(tiles.begin(), tiles.end(), [](const PrefillTile& a, const PrefillTile& b) { return a.pos0 + a.n_rows > b.pos0 + b.n_rows; });
 }
 
 void build_decode_plan(const int32_t* ctx_lens, int n_seqs, int n_kv, int n_ctas_target, int force_splits, DecodePlan& out) {
@@ -424,9 +434,8 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         o_cnt = put(zero_counters_.data(), zero_counters_.size());     // merge counters start every step at zero
     }
     if (!in.decode) {
-        // heaviest query tiles (most visible keys) first: the causal triangle otherwise leaves a long tail of big CTAs
         sorted_tiles_ = in.tiles;
-        std::stable_sort(sorted_tiles_.begin(), sorted_tiles_.end(), [](const PrefillTile& a, const PrefillTile& b) { return a.pos0 + a.n_rows > b.pos0 + b.n_rows; });
+        sort_prefill_tiles(sorted_tiles_);
         o_tiles = put(sorted_tiles_.data(), sorted_tiles_.size() * 4);
     }
     cuda_check(cudaMemcpyAsync(d_meta_, h_meta_, w * 4, cudaMemcpyHostToDevice, stream), "meta H2D");
@@ -453,7 +462,7 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
     // fp8 weights: every projection reads its input as e4m3 rows + per-row scales, quantised by one kernel right before the GEMM
     const bool w8 = cfg.w_fp8();
     auto quant = [&](const ProjInput& a) { if (a.q) { cuda_check(launch_quant_rows_e4m3(a.x, a.q, a.sc, T, a.cols, stream), "fp8 quantise"); MARK(14); } };
-    auto cap = [&](int bn) { return w8 ? std::min(bn, 128) : bn; };      // fp8 tiles are at most 128 wide (registers)
+    auto cap = [&](int bn) { return w8 ? std::min(bn, W8_MAX_BN) : bn; };
     // decode-sized batches (one or, opt-in, two 128-row tiles; fp8: one, the promoted fp8 fragment leaves no registers for a second)
     const bool use_sk = opt.streamk && T <= (w8 ? 128 : std::min(256, std::max(128, opt.sk_max_rows)));
     const int sk_rows = T > 128 ? 256 : 128;
@@ -572,8 +581,8 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                 cuda_check(launch_ar_resid_bf16(comm->d_peer_sym(b), tp, x_, T, H, stream), "allreduce+resid");
             }
         };
-        const int bn_qkv = cap(pick_bn(T, qkvd, opt.bn_qkv)), bn_o = cap(pick_bn(T, H, opt.bn_o));
-        const int bn_gu = cap(pick_bn(T, 2 * F, opt.bn_gu)), bn_down = cap(pick_bn(T, H, opt.bn_down));
+        const int bn_qkv = pick_bn(T, qkvd, sm_count, opt.bn_qkv, w8), bn_o = pick_bn(T, H, sm_count, opt.bn_o, w8);
+        const int bn_gu = pick_bn(T, 2 * F, sm_count, opt.bn_gu, w8), bn_down = pick_bn(T, H, sm_count, opt.bn_down, w8);
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
             cuda_check(launch_rmsnorm(x_, ly.ln1, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
@@ -600,7 +609,7 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
             cuda_check(launch_rmsnorm(xs_, final_norm, xsn_, S, H, cfg.rms_eps, stream), "final norm");
         }
         MARK(11);
-        const int bn_lm = pick_bn(S, V, opt.bn_lm);
+        const int bn_lm = pick_bn(S, V, sm_count, opt.bn_lm);
         const int n_tiles = gemm_n_tiles(V, bn_lm);
         GemmParams gl{}; gl.M = S; gl.N = V; gl.K = H; gl.logits = logits_out; gl.ldl = V; gl.amax_val = amax_val_; gl.amax_idx = amax_idx_;
         if (!in.mask_slots.empty()) {          // constrained rows: the arg-max runs over their state's allowed tokens, on every vocabulary shard

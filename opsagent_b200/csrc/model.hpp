@@ -48,6 +48,13 @@ struct DecodePlan {
 };
 // contiguous, balanced partition of all (sequence, kv head) page lists over n_ctas CTAs
 void build_decode_plan(const int32_t* ctx_lens, int n_seqs, int n_kv, int n_ctas_target, int force_splits, DecodePlan& out);
+// the prefill tiles of `n_rows` new rows of sequence `seq` at token-batch row `row0`, the first at position `pos0`
+void append_prefill_tiles(std::vector<PrefillTile>& tiles, int seq, int row0, int pos0, int n_rows);
+// the order the prefill-attention grid runs its tiles in: heaviest (most visible keys) first
+void sort_prefill_tiles(std::vector<PrefillTile>& tiles);
+constexpr int W8_MAX_BN = 128;      // fp8 GEMM tiles are at most 128 wide (registers)
+// BLOCK_N of a tile-path GEMM [M, N] on sm_count SMs (override_bn in {32, 64, 128, 256} wins); fp8 operands cap it at W8_MAX_BN
+int pick_bn(int M, int N, int sm_count, int override_bn, bool fp8 = false);
 
 class DeviceModel {
 public:
@@ -93,7 +100,6 @@ private:
     void commit(WeightMat& w);
     void load_checkpoint(const std::string& path);     // overwrite the seeded tensors with this rank's slices of an HF checkpoint
     void make_weight_maps(WeightMat& w);
-    int pick_bn(int M, int N, int override_bn) const;
     void* dmalloc(size_t bytes);
     std::vector<void*> allocs_;
     // activations

@@ -459,6 +459,23 @@ def test_http_front_serves_the_perf_stats_endpoints():
     srv.shutdown()
 
 
+# ---- the tile-path GEMMs' BLOCK_N (pick_bn, host only) ----
+def test_pick_bn_choices():
+    from opsagent_b200 import _lib
+    L = _lib.load()
+
+    def pick(M, N, sms=132, override=0, fp8=0):
+        return L.oa_host_pick_bn(M, N, sms, override, fp8)
+
+    assert pick(257, 2048) == 32                   # Llama-3.2-1B's o at T = 257: 3 row tiles x 64 column tiles >= 132 SMs
+    assert pick(129, 2048) == 32 and pick(129, 3072) == 64 and pick(129, 16384) == 128     # two row tiles: about half the SMs
+    assert pick(8192, 2048) == 128 and pick(1000, 4096) == 128 and pick(1000, 2048) == 64
+    for bn in (32, 64, 128, 256):                  # an override wins; fp8 tiles are at most 128 wide
+        assert pick(8192, 8192, override=bn) == bn and pick(8192, 8192, override=bn, fp8=1) == min(bn, 128)
+    assert pick(8192, 8192, override=48) == 128    # not a BLOCK_N: ignored
+    assert pick(1, 64) == 32 and pick(1, 64, fp8=1) == 32
+
+
 # ---- stream-K unit plan: the invariants the fused SwiGLU epilogue and the consumers rely on (host only) ----
 @pytest.mark.parametrize("N,K,G", [(28672, 4096, 148), (6144, 4096, 148), (4096, 4096, 148), (4096, 14336, 148),     # Llama-3-8B decode projections
                                    (7168, 8192, 148), (1280, 8192, 148), (8192, 1024, 148), (8192, 3584, 148),     # Llama-3-70B TP=8 shards
