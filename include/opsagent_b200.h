@@ -215,6 +215,28 @@ OA_API int oa_k_step_attention(const void* q, void* out, const void* kv_cache, i
                                int32_t n_heads, int32_t n_kv, int32_t head_dim, float k_scale, float v_scale, void* stream);
 /* out [T, H] = table [vocab, H] rows of ids [T] (device); an id outside [0, vocab) reads row 0 */
 OA_API int oa_k_embed_gather(const int32_t* ids, const void* table, void* out, int32_t T, int32_t H, int32_t vocab, void* stream);
+/* The tensor-parallel collectives of DeviceModel::forward on one GPU (test entry points, synchronous).  Each collective reaches its peers through
+ * a device table of pointers; here the t entries point at t local buffers, and ranks 0 .. t-1 run one after another on one stream, each with
+ * the arguments that rank has on t GPUs.  Arrays of t device pointers are host arrays.  t outside 2..8 or a row length (H, K) that is not a
+ * multiple of 8 returns OA_ERR_BAD_REQUEST, as does a launcher's refusal.
+ * Decode o / down finish: per rank r, the stream-K GEMM of A[r] [M, K] by B[r] [H, K] (bf16; two 128-row slots when M > 128), its fp32 or
+ * (bf16_partials) bf16 sum into partial[r] [M, H] with rank r's "buffer written" signal, then x[r] [M, H] += the rank-ordered sum of every
+ * partial and xn[r] = rmsnorm(x[r]) * gain, after rank r's wait for the t signals.  flags: device uint32 [t][8] (rank p's flags are row p);
+ * launch i uses epoch + i (wrapping).  The consumers of a launch run only once every one of the t x t flags shows its epoch, otherwise the
+ * call returns OA_ERR_INTERNAL (oa_last_error names the flag).  `launches` repeats everything on the same flags and done counters. */
+OA_API int oa_k_tp_row_parallel(int32_t t, const void* const* A, const void* const* B, int32_t M, int32_t H, int32_t K, int32_t block_n,
+                                int32_t n_ctas, int32_t bf16_partials, void* const* partial, void* const* x, void* const* xn, const void* gain,
+                                float eps, uint32_t* flags, uint32_t epoch, int32_t launches, void* stream);
+/* Prefill all-reduce: x[r] [T, H] += the rank-ordered sum of the bf16 partials partial[·] [T, H], one-shot, or two-shot (rank r reduces
+ * slice r of the flat T x H / 8 16-byte vectors into x[r] and gather[r], then copies every other rank's slice from gather[·]). */
+OA_API int oa_k_tp_allreduce_prefill(int32_t t, void* const* partial, void* const* x, void* const* gather, int32_t T, int32_t H, int32_t two_shot,
+                                     void* stream);
+/* Vocab-parallel LM head: shard r = B rows [r V/t, (r+1) V/t) of B [V, K].  Its logits (optional: logits [M, V] at column r V/t), its
+ * (max, lowest global id) per row into pairs[r] ({float, int32} [M]), then ids [M] = the best pair over the shards (ties: lowest id).
+ * block_n 0 = the engine's choice for one shard.  A masked row (mask table as oa_k_gemm_logits_masked, bit = global id) with nothing
+ * allowed gives (-inf, r V/t) on shard r and id 0.  V % t and (V / t) % 8 must be 0. */
+OA_API int oa_k_tp_lm_head_argmax(int32_t t, const void* A, const void* B, int32_t M, int32_t V, int32_t K, int32_t block_n, const uint32_t* mask_table,
+                                  const int32_t* mask_slot, int32_t mask_words, float* logits, void* const* pairs, int32_t* ids, void* stream);
 /* ---- host-only logic, callable without a GPU (CPU tests) ---- */
 /* BLOCK_N of the engine's tile-path GEMM [M, N] on sm_count SMs (pick_bn; override_bn in {32, 64, 128, 256} wins, fp8 != 0 caps it at 128) */
 OA_API int32_t oa_host_pick_bn(int32_t M, int32_t N, int32_t sm_count, int32_t override_bn, int32_t fp8);

@@ -39,6 +39,7 @@ SYMBOLS = [
     "oa_k_quant_rows_e4m3", "oa_k_gemm_fp8", "oa_k_gemm_streamk_fp8",
     "oa_k_sk_row_parallel", "oa_k_sk_swiglu", "oa_k_sk_qkv_rope", "oa_k_kv_write", "oa_k_decode_attention", "oa_k_gemm_logits_masked",
     "oa_k_prefill_gemm", "oa_k_step_attention", "oa_k_embed_gather", "oa_host_pick_bn",
+    "oa_k_tp_row_parallel", "oa_k_tp_allreduce_prefill", "oa_k_tp_lm_head_argmax",
 ]
 
 _lib = None
@@ -94,6 +95,11 @@ def load() -> C.CDLL:
     L.oa_k_step_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, f32, f32, vp]; L.oa_k_step_attention.restype = C.c_int
     L.oa_k_embed_gather.argtypes = [vp, vp, vp, i32, i32, i32, vp]; L.oa_k_embed_gather.restype = C.c_int
     L.oa_host_pick_bn.argtypes = [i32, i32, i32, i32, i32]; L.oa_host_pick_bn.restype = i32
+    vpp = C.POINTER(vp)                    # host array of device pointers
+    L.oa_k_tp_row_parallel.argtypes = [i32, vpp, vpp, i32, i32, i32, i32, i32, i32, vpp, vpp, vpp, vp, f32, vp, C.c_uint32, i32, vp]
+    L.oa_k_tp_row_parallel.restype = C.c_int
+    L.oa_k_tp_allreduce_prefill.argtypes = [i32, vpp, vpp, vpp, i32, i32, i32, vp]; L.oa_k_tp_allreduce_prefill.restype = C.c_int
+    L.oa_k_tp_lm_head_argmax.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, i32, vp, vpp, vp, vp]; L.oa_k_tp_lm_head_argmax.restype = C.c_int
     L.oa_host_apply_chat_template.argtypes = [C.c_char_p, C.POINTER(OaMsg), i32, vp, i32, C.POINTER(i32)]; L.oa_host_apply_chat_template.restype = C.c_int
     L.oa_host_bpe_encode.argtypes = [C.c_char_p, C.c_char_p, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_encode.restype = C.c_int
     L.oa_host_bpe_decode.argtypes = [C.c_char_p, vp, i32, vp, i32, C.POINTER(i32)]; L.oa_host_bpe_decode.restype = C.c_int

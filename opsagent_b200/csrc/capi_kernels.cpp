@@ -69,6 +69,20 @@ int decode_attention(const void* q, void* out, const KvLayout& kv, const int32_t
 int prefill_attention(const void* q, void* out, const KvLayout& kv, const int32_t* block_tables, int32_t max_pages_per_seq, const int32_t* ctx_lens,
                       const int32_t* q_lens, int32_t seq0, int32_t n_seqs, int32_t n_heads, cudaStream_t s);
 int sm_count() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n > 0 ? n : 132; }
+
+// A device table of t pointers, the way a tensor-parallel collective reaches its peers' buffers (TpComm's d_peer_sym / d_peer_arg).  On one
+// GPU the t entries are t local buffers, and the kernel launched with rank r's arguments does what rank r does on t GPUs.
+struct PeerTable {
+    void* h[TP_MAX] = {};
+    DevBuf d{sizeof(h)};
+    PeerTable(const void* const* p, int t, size_t stride = 0) {
+        for (int r = 0; r < t; ++r) h[r] = stride ? (char*)const_cast<void*>(p[0]) + r * stride : const_cast<void*>(p[r]);
+        if (d.p && cudaMemcpy(d.p, h, sizeof(h), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d.p); d.p = nullptr; }
+    }
+    void* const* get() const { return (void* const*)d.p; }
+};
+// the tensor-parallel shapes ModelConfig accepts (config.hpp): 2..8 ranks, rows of a multiple of 8 elements
+bool tp_shape_ok(int t, int H) { return t >= 2 && t <= TP_MAX && H > 0 && H % 8 == 0; }
 }  // namespace
 
 // test-only: materialise the deterministic fixed-order sum of stream-K partials as fp32 [M,N]
@@ -335,6 +349,94 @@ int oa_k_decode_attention(const void* q, void* out, const void* kv_cache, int32_
     const bool kv8 = k_scale > 0.f;
     return decode_attention(q, out, one_layer_kv(kv_cache, num_pages, n_kv, head_dim, kv8 ? &k_scale : nullptr, kv8 ? &v_scale : nullptr), block_tables,
                             max_pages_per_seq, ctx_lens, n_seqs, n_heads, n_ctas_target, 0, merge_inline != 0, launches, (cudaStream_t)stream);
+}
+
+// ---- the tensor-parallel collectives, t ranks emulated one after another on one stream (see the header) ----
+int oa_k_tp_row_parallel(int32_t t, const void* const* A, const void* const* B, int32_t M, int32_t H, int32_t K, int32_t block_n, int32_t n_ctas,
+                         int32_t bf16_partials, void* const* partial, void* const* x, void* const* xn, const void* gain, float eps, uint32_t* flags,
+                         uint32_t epoch, int32_t launches, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!tp_shape_ok(t, H) || M <= 0 || launches < 1) return OA_ERR_BAD_REQUEST;
+    CUtensorMap tmA[TP_MAX], tmB[TP_MAX];
+    for (int r = 0; r < t; ++r) if (!proj_maps(&tmA[r], &tmB[r], A[r], B[r], false, M, H, K, block_n)) return OA_ERR_INTERNAL;
+    // one workspace for every rank: rank r + 1's GEMM runs after rank r's reduce in stream order
+    SkSetup st(H, K, block_n, n_ctas, M > 128 ? 256 : 128, false, s);
+    DevBuf done((size_t)TP_MAX * 64);                     // each rank's "CTAs finished" counter, on its own 64 bytes as TpComm allocates it
+    const void* fbase = flags;
+    PeerTable parts(partial, t), peer_flags(&fbase, t, 8 * sizeof(uint32_t));
+    if (!st.ok() || !done.p || !parts.get() || !peer_flags.get() || cudaMemsetAsync(done.p, 0, (size_t)TP_MAX * 64, s) != cudaSuccess) return OA_ERR_INTERNAL;
+    auto signal = [&](int r, uint32_t e) {
+        return TpComm::Signal{(uint32_t* const*)peer_flags.get(), flags + r * 8, (unsigned int*)done.p + r * 16, r, t, e};
+    };
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < launches; ++i) {
+        const uint32_t ep = epoch + (uint32_t)i;
+        for (int r = 0; r < t && e == cudaSuccess; ++r) {
+            const TpComm::Signal sg = signal(r, ep);
+            e = launch_gemm_streamk(&tmA[r], &tmB[r], M, H, K, st.sk, s);
+            if (e == cudaSuccess)
+                e = bf16_partials ? launch_sk_reduce_bf16(st.sk, partial[r], M, H, s, &sg) : launch_sk_reduce_f32(st.sk, (float*)partial[r], M, H, s, &sg);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) return rc_launch(e);
+        // every consumer below waits for the t signals of this epoch: launch none of them unless all t x t flags already show it
+        uint32_t h[TP_MAX * 8];
+        if (cudaMemcpy(h, flags, (size_t)t * 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess) return OA_ERR_INTERNAL;
+        for (int p = 0; p < t; ++p)
+            for (int r = 0; r < t; ++r)
+                if (h[p * 8 + r] != ep)
+                    return fail_host(OA_ERR_INTERNAL, "tp row-parallel: launch " + std::to_string(i) + ", rank " + std::to_string(r) + " did not signal rank " +
+                                                          std::to_string(p) + " (flag " + std::to_string(h[p * 8 + r]) + ", epoch " + std::to_string(ep) + ")");
+        for (int r = 0; r < t && e == cudaSuccess; ++r) {
+            const TpComm::Signal sg = signal(r, ep);
+            e = bf16_partials ? launch_ar_resid_rmsnorm_bf16in(parts.get(), t, x[r], gain, xn[r], M, H, eps, s, &sg)
+                              : launch_ar_resid_rmsnorm(parts.get(), t, x[r], gain, xn[r], M, H, eps, s, &sg);
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_tp_allreduce_prefill(int32_t t, void* const* partial, void* const* x, void* const* gather, int32_t T, int32_t H, int32_t two_shot, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!tp_shape_ok(t, H) || T < 0 || (two_shot && !gather)) return OA_ERR_BAD_REQUEST;
+    PeerTable parts(partial, t);
+    if (!parts.get()) return OA_ERR_INTERNAL;
+    cudaError_t e = cudaSuccess;
+    if (!two_shot) {
+        for (int r = 0; r < t && e == cudaSuccess; ++r) e = launch_ar_resid_bf16(parts.get(), t, x[r], T, H, s);
+    } else {                                              // stream order stands in for the engine's barrier between the two halves
+        PeerTable gath(gather, t);
+        if (!gath.get()) return OA_ERR_INTERNAL;
+        for (int r = 0; r < t && e == cudaSuccess; ++r) e = launch_ar2_reduce_scatter(parts.get(), t, r, x[r], gather[r], T, H, s);
+        for (int r = 0; r < t && e == cudaSuccess; ++r) e = launch_ar2_all_gather(gath.get(), t, r, x[r], T, H, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);      // before gath's table is freed
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
+}
+
+int oa_k_tp_lm_head_argmax(int32_t t, const void* A, const void* B, int32_t M, int32_t V, int32_t K, int32_t block_n, const uint32_t* mask_table,
+                           const int32_t* mask_slot, int32_t mask_words, float* logits, void* const* pairs, int32_t* ids, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!tp_shape_ok(t, K) || M <= 0 || V <= 0 || V % t || (V / t) % 8) return OA_ERR_BAD_REQUEST;
+    const int Vs = V / t, bn = block_n ? block_n : pick_bn(M, Vs, sm_count(), 0), nt = gemm_n_tiles(Vs, bn);
+    PeerTable pt(pairs, t);
+    DevBuf av((size_t)t * M * nt * 4), ai((size_t)t * M * nt * 4);       // each shard's per-tile (max, arg-max): the engine's amax_val_ / amax_idx_
+    if (!pt.get() || !av.p || !ai.p) return OA_ERR_INTERNAL;
+    cudaError_t e = cudaSuccess;
+    for (int r = 0; r < t && e == cudaSuccess; ++r) {
+        CUtensorMap tmA, tmB;
+        if (!proj_maps(&tmA, &tmB, A, (const char*)B + (size_t)r * Vs * K * 2, false, M, Vs, K, bn)) return OA_ERR_INTERNAL;
+        GemmParams p{}; p.M = M; p.N = Vs; p.K = K; p.logits = logits ? logits + (size_t)r * Vs : nullptr; p.ldl = V;
+        p.amax_val = (float*)av.p + (size_t)r * M * nt; p.amax_idx = (int*)ai.p + (size_t)r * M * nt;
+        if (mask_table) { p.mask_table = mask_table; p.mask_slot = mask_slot; p.mask_words = mask_words; p.col_offset = r * Vs; }
+        e = launch_gemm(&tmA, &tmB, p, EPI_LOGITS, bn, s);
+        if (e == cudaSuccess) e = launch_argmax_reduce_pair(p.amax_val, p.amax_idx, M, nt, r * Vs, pairs[r], s);
+    }
+    if (e == cudaSuccess) e = launch_ar_argmax(pt.get(), t, M, ids, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return rc_launch(e);
 }
 
 }  // extern "C"

@@ -29,6 +29,13 @@ PRESETS = {
     "qwen2.5-32b": (5120, 40, 8, 128, 27648, True),
     "llama-3-70b": (8192, 64, 8, 128, 28672, False),
 }
+# one tensor-parallel rank's column-parallel layout (its heads and its ffn shard; hidden stays whole): the same qkv and gate/up kernels at
+# shapes the single-GPU presets never make.  Not in PRESETS: the fused o / down finishers never run under tensor parallelism.
+TP_RANKS = {
+    "qwen2.5-32b/tp4": (5120, 10, 2, 128, 6912, True),
+    "llama-3-70b/tp8": (8192, 8, 1, 128, 3584, False),
+}
+LAYOUTS = {**PRESETS, **TP_RANKS}
 
 # Bounds and exact-match floors: tests/kernel_ref.py (measured on an H100 SXM, 132 SMs, default power limit).  The whole file runs in about
 # 30 s on that GPU.
@@ -88,7 +95,7 @@ def proj(L, preset, kind, N=None, K=None):
         if any(k[0] != preset for k in _CACHE):
             _CACHE.clear(); torch.cuda.empty_cache()
         if N is None:
-            H, nh, nkv, D, F, _ = PRESETS[preset]
+            H, nh, nkv, D, F, _ = LAYOUTS[preset]
             N, K = {"o": (H, nh * D), "down": (H, F), "qkv": ((nh + 2 * nkv) * D, H), "gu": (2 * F, H)}[kind]
         _CACHE[key] = Proj(L, N, K, zlib.crc32(f"{preset}/{kind}".encode()) & 0xFFFF)
     return _CACHE[key]
@@ -162,7 +169,7 @@ def gu_reference(P, M, fp8):
 
 # + a small gate/up (N = 1024, K = 4096: 512 k-block units on 132 SMs) whose tiles are cut into up to 17 pieces.  At the presets' shapes
 # every CTA owns more units than a tile has, so no tile has more than two pieces there and the finisher's loop over further pieces never runs.
-@pytest.mark.parametrize("preset", list(PRESETS) + ["many-pieces"])
+@pytest.mark.parametrize("preset", list(LAYOUTS) + ["many-pieces"])
 def test_swiglu_matches_fp64(L, sms, preset):
     P = proj(L, preset, "gu", *((1024, 4096) if preset == "many-pieces" else (None, None)))
     for fp8 in (False, True):
@@ -322,9 +329,9 @@ def qkv_check(P, Q, M, q_out, cache, kvs, fp8, what, min_equal):
             assert frac >= min_equal, f"{name}{tag}: {what}: only {frac:.5f} of the bytes equal the rounded reference's"
 
 
-@pytest.mark.parametrize("preset", PRESETS)
+@pytest.mark.parametrize("preset", LAYOUTS)
 def test_qkv_rope_kv_write_matches_fp64(L, sms, preset):
-    H, nh, nkv, D, F, bias = PRESETS[preset]
+    H, nh, nkv, D, F, bias = LAYOUTS[preset]
     P = proj(L, preset, "qkv")
     Q = QkvCase(preset, nh, nkv, D, bias)
     for fp8 in (False, True):
@@ -341,7 +348,10 @@ def test_qkv_rope_kv_write_matches_fp64(L, sms, preset):
                 what = f"{preset} cache {kvs or 'bf16'} path {path} bn {bn} n_ctas {G} M {M}"
                 rc, q_out, cache = qkv_run(L, P, Q, M, path, bn, G, kvs, fp8)
                 assert rc == 0, (what, rc, _lib.last_error())
-                qkv_check(P, Q, M, q_out, cache, kvs, fp8, what, MIN_EQUAL_FP8 if fp8 else MIN_EQUAL)
+                # the K / V rows of one or two tokens of a tensor-parallel rank (one or two kv heads) are 128 to 256 values: too few for
+                # an exact-match floor (two misses fail 0.99).  Every preset's rows have at least 512.
+                floor = (MIN_EQUAL_FP8 if fp8 else MIN_EQUAL) if M * nkv * D >= 512 else 0.0
+                qkv_check(P, Q, M, q_out, cache, kvs, fp8, what, floor)
     report(preset)
 
 
@@ -535,7 +545,8 @@ def attn_ref64(q, K, V, bt, ctx, nh, nkv, D):
 
 
 @pytest.mark.parametrize("kvs", KV_SCALES)
-@pytest.mark.parametrize("nh,nkv,D", [(8, 8, 128), (32, 8, 64), (32, 8, 128), (40, 8, 128), (64, 8, 128)])    # GQA groups 1, 4, 4, 5, 8
+@pytest.mark.parametrize("nh,nkv,D", [(8, 8, 128), (32, 8, 64), (32, 8, 128), (40, 8, 128), (64, 8, 128),    # GQA groups 1, 4, 4, 5, 8
+                                      (10, 2, 128), (8, 1, 128)])       # one tensor-parallel rank of Qwen2.5-32B t = 4, Llama-3-70B t = 8
 def test_decode_attention_in_kernel_merge(L, sms, nh, nkv, D, kvs):
     n = len(CTX); maxp = max((c + 63) // 64 for c in CTX); num_pages = sum((c + 63) // 64 for c in CTX) + 7
     g = torch.Generator(device="cpu").manual_seed(nh + D)

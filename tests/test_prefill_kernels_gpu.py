@@ -247,7 +247,8 @@ def test_engine_block_n_choices_cover_32_64_128(L, sms):
 FRESH = [(0, n) for n in (1, 63, 64, 65, 127, 128, 129, 1536, 8192)]
 CONT = [(100, 28), (100, 300), (1540, 1), (1540, 700), (4095, 1), (4095, 129), (4095, 2000), (12000, 385), (16383, 1), (1, 127), (4033, 300)]
 SEQS = FRESH + CONT
-HEADS = [(32, 8, 64), (32, 8, 128), (40, 8, 128), (64, 8, 128)]
+HEADS = [(32, 8, 64), (32, 8, 128), (40, 8, 128), (64, 8, 128),
+         (10, 2, 128), (8, 1, 128)]     # one tensor-parallel rank of Qwen2.5-32B at t = 4 and of Llama-3-70B at t = 8
 N_DECODE = [1, 37, 128]
 LARGE_POOL = {False: 10000, True: 20000}     # pages of the 32/8/128 cache: more than 2 GiB, so byte offsets pass 2^31
 
