@@ -12,9 +12,6 @@
 
 namespace oa {
 
-void cuda_check(cudaError_t e, const char* what) {
-    if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-}
 static void tmap_check(int r, const char* what) {
     if (r != 0) throw std::runtime_error(std::string("cuTensorMapEncodeTiled failed for ") + what + " (code " + std::to_string(r) + ")");
 }
@@ -384,15 +381,6 @@ void build_decode_plan(const int32_t* ctx_lens, int n_seqs, int n_kv, int n_ctas
     out.cta_ptr[(size_t)n_ctas] = (int32_t)k;
 }
 
-// cuda_check labels of the two row-parallel projections on the stream-K path and of the norm that follows each
-struct RowParallelLabels { const char *clusterk, *fused, *gemm, *norm, *resid, *nvls_part, *nvls_ar, *bf16_part, *f32_part, *ar; };
-static const RowParallelLabels kOLabels = {
-    "o gemm + residual (cluster split-K)", "o gemm + residual (stream-K)", "o gemm (stream-K)", "rmsnorm2", "resid+rmsnorm2", "o partial -> multicast buffer",
-    "in-switch allreduce+resid+rmsnorm2", "o partial -> symmetric buffer (bf16)", "o partial -> symmetric buffer", "allreduce+resid+rmsnorm2"};
-static const RowParallelLabels kDownLabels = {
-    "down gemm + residual (cluster split-K)", "down gemm + residual (stream-K)", "down gemm (stream-K)", "rmsnorm1", "resid+rmsnorm1", "down partial -> multicast buffer",
-    "in-switch allreduce+resid+rmsnorm1", "down partial -> symmetric buffer (bf16)", "down partial -> symmetric buffer", "allreduce+resid+rmsnorm1"};
-
 void DeviceModel::forward(const StepInput& in, float* logits_out) {
     const int T = (int)in.tokens.size(), S = (int)in.sample_rows.size();
     // all projection sizes below are this rank's shard (== the global sizes when tp == 1)
@@ -457,7 +445,7 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         cudaEventRecord(ev_all[ek++], stream);
     }
     auto MARK = [&](int id) { if (profile_all && ek < ev_all.size()) { ev_ids[ek] = id; cudaEventRecord(ev_all[ek++], stream); } };
-    const float scale_log2e = (1.0f / std::sqrt((float)D)) * 1.4426950408889634f;
+    const Mark mark = profile_all ? Mark(MARK) : Mark();       // the stage functions' marks
     cuda_check(launch_embed_gather(d_tok, embed, x_, T, H, cfg.vocab, stream), "embed"); MARK(0);
     // fp8 weights: every projection reads its input as e4m3 rows + per-row scales, quantised by one kernel right before the GEMM
     const bool w8 = cfg.w_fp8();
@@ -466,32 +454,24 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
     // decode-sized batches (one or, opt-in, two 128-row tiles; fp8: one, the promoted fp8 fragment leaves no registers for a second)
     const bool use_sk = opt.streamk && T <= (w8 ? 128 : std::min(256, std::max(128, opt.sk_max_rows)));
     const int sk_rows = T > 128 ? 256 : 128;
+    // rows 0 .. n_dec-1: decode attention, cut items merged inside the kernel by the CTA finishing their last piece; then the prefill tiles
+    const DecodeAttnParams dec{q_, attn_.x, d_bt, d_ctx, max_pages_per_seq, reinterpret_cast<const DecodeSeg*>(d_meta_ + o_segs), d_meta_ + o_ptr,
+                               n_dec > 0 ? (int)plan_.cta_ptr.size() - 1 : 0, part_o_, part_ml_, d_meta_ + o_cnt, 0, nh, nkv, 0.f};
+    const PrefillAttnParams pre{q_, attn_.x, d_bt, max_pages_per_seq, reinterpret_cast<const PrefillTile*>(d_meta_ + o_tiles),
+                                in.decode ? 0 : (int)in.tiles.size(), 0, nh, nkv, 0.f};
     auto attention = [&](int l) {
         if (profile_attn) cudaEventRecord(ev[2 * l], stream);
-        if (n_dec > 0) {
-            DecodeAttnParams a{}; a.q = q_; a.out = attn_.x; a.block_tables = d_bt; a.ctx_lens = d_ctx; a.max_pages_per_seq = max_pages_per_seq;
-            a.segs = reinterpret_cast<const DecodeSeg*>(d_meta_ + o_segs); a.cta_seg_ptr = d_meta_ + o_ptr; a.n_ctas = (int)plan_.cta_ptr.size() - 1;
-            a.part_o = part_o_; a.part_ml = part_ml_; a.layer = l; a.n_heads = nh; a.n_kv = nkv; a.scale_log2e = scale_log2e;
-            a.merge_counters = d_meta_ + o_cnt;      // cut items are merged inside the kernel by the CTA finishing their last piece
-            cuda_check(launch_decode_attention(&tm_kv, kv, a, stream), "decode attention"); MARK(4);
-        }
-        if (!in.decode && !in.tiles.empty()) {     // mixed step: both kernels, disjoint rows of q_/attn_
-            PrefillAttnParams a{}; a.q = q_; a.out = attn_.x; a.block_tables = d_bt; a.max_pages_per_seq = max_pages_per_seq;
-            a.tiles = reinterpret_cast<const PrefillTile*>(d_meta_ + o_tiles); a.n_tiles = (int)in.tiles.size();
-            a.layer = l; a.n_heads = nh; a.n_kv = nkv; a.scale_log2e = scale_log2e;
-            cuda_check(launch_prefill_attention(&tm_kv, kv, a, stream), "prefill attention");
-            MARK(4);
-        }
+        step_attention(&tm_kv, kv, dec, pre, l, stream, mark);
         if (profile_attn) cudaEventRecord(ev[2 * l + 1], stream);
     };
     if (use_sk) {
         // decode-sized batch: persistent stream-K projections (fp32 partials) + fused consumers
         auto bn_of = [&](int o) { return cap(sk_rows == 256 ? 128 : ((o == 64 || o == 128 || o == 256) ? o : sk_bn_)); };      // two row tiles need BN <= 128 (registers)
-        auto with_pf = [&](StreamK k) { k.l2_prefetch_units = std::max(0, opt.sk_l2_prefetch_kb * 1024 / (k.bn * 128)); return k; };
-        const StreamK sk_qkv = make_streamk(sk_ws_, qkvd, H, bn_of(opt.sk_bn_qkv), sk_G_, sk_rows, w8), sk_o = make_streamk(sk_ws_, H, qd, bn_of(opt.sk_bn_o), sk_G_, sk_rows, w8);
-        const StreamK sk_gu = make_streamk(sk_ws_, 2 * F, H, bn_of(opt.sk_bn_gu), sk_G_, sk_rows, w8), sk_dn = make_streamk(sk_ws_, H, F, bn_of(opt.sk_bn_down), sk_G_, sk_rows, w8);
+        auto sk_for = [&](int N, int K, int o) {        // the GEMM prefetches its first weight tiles into L2
+            StreamK k = make_streamk(sk_ws_, N, K, bn_of(o), sk_G_, sk_rows, w8); k.l2_prefetch_units = std::max(0, opt.sk_l2_prefetch_kb * 1024 / (k.bn * 128)); return k;
+        };
+        const StreamK sk_qkv = sk_for(qkvd, H, opt.sk_bn_qkv), sk_o = sk_for(H, qd, opt.sk_bn_o), sk_gu = sk_for(2 * F, H, opt.sk_bn_gu), sk_dn = sk_for(H, F, opt.sk_bn_down);
         cuda_check(launch_rmsnorm(x_, layers[0].ln1, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
-        const StreamK pf_qkv = with_pf(sk_qkv), pf_o = with_pf(sk_o), pf_gu = with_pf(sk_gu), pf_dn = with_pf(sk_dn);
         // qkv / o / down epilogues finished inside the GEMM (same conditions as the fused SwiGLU; every projection at BN = 128, tile counts within the flag arrays)
         const bool fuse_ok = sk_rows == 128 && sk_G_ <= sm_count && sk_qkv.bn == 128 && sk_o.bn == 128 && sk_dn.bn == 128 &&
                               sk_qkv.n_tiles <= SK_MAX_FLAG_TILES && sk_o.n_tiles <= SK_MAX_FLAG_TILES && (D == 64 || D == 128);
@@ -502,76 +482,52 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         const int ck_o = (sk_rows == 128 && (opt.sk_clusterk & 2) && !use_tp) ? clusterk_pick(H, qd, sm_count, opt.sk_clusterk_min_fill) : 0;
         const int ck_dn = (sk_rows == 128 && (opt.sk_clusterk & 4) && !use_tp) ? clusterk_pick(H, F, sm_count, opt.sk_clusterk_min_fill) : 0;
         const bool fuse_swiglu = opt.sk_fuse_swiglu && !w8 && sk_rows == 128 && sk_gu.bn == 128 && sk_G_ <= sm_count && sk_gu.n_tiles <= SK_MAX_FLAG_TILES;
+        // each projection's finishing path (stages.hpp): cluster split-K, fused stream-K finisher, or GEMM + consumer
+        const int path_qkv = ck_qkv ? ck_qkv : fuse_rope, path_o = ck_o ? ck_o : fuse_o, path_dn = ck_dn ? ck_dn : fuse_dn, path_gu = fuse_swiglu;
+        auto proj = [&](int path, const ProjInput& a, const WeightMat& w, const StreamK& sk, int flag_slot) {
+            return SkGemm{path, a.map(), w.map(path == 0 ? sk.bn : 128), T, w.N, w.K, sk, a.w8(w), tile_flags_ + flag_slot * SK_MAX_FLAG_TILES};
+        };
         // row-parallel projection (o, down): x += a . w^T, then xn = rmsnorm(x) * gain
-        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int K, int ck, bool fused, const StreamK& sk, const StreamK& pf, int flag_slot,
-                                const void* gain, int mark, const RowParallelLabels& lb) {
-            if (ck || fused) {
-                if (ck) cuda_check(launch_gemm_clusterk_resid(&a.tm, w.map(128), T, H, K, ck, x_, H, stream), lb.clusterk);
-                else cuda_check(launch_gemm_streamk_resid(a.map(), w.map(128), T, H, K, pf, x_, H, tile_flags_ + flag_slot * SK_MAX_FLAG_TILES, stream, a.w8(w)), lb.fused);
-                MARK(mark);
-                cuda_check(launch_rmsnorm_wide(x_, gain, xn_.x, T, H, cfg.rms_eps, stream), lb.norm); MARK(7);
+        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int path, const StreamK& sk, int flag_slot, const void* gain, const RowParallelOp& op) {
+            const SkGemm g = proj(path, a, w, sk, flag_slot);
+            if (!use_tp) return finish_row_parallel(g, x_, gain, xn_.x, cfg.rms_eps, op, stream, mark);
+            // all-reduce the rank partials over NVLink peer memory, then residual + norm
+            const int b = comm->next_buffer();
+            const TpComm::Signal sg = comm->next_signal();     // "buffer written" handshake rides on the two kernels: no barrier launch
+            if (comm->nvls() && T <= 128) {
+                char* loc = reinterpret_cast<char*>(comm->nvls_local());
+                cuda_check(launch_gemm_streamk(g.tmA, g.tmB, T, H, g.K, sk, stream, g.w8), op.gemm); MARK(op.mark);
+                cuda_check(launch_sk_reduce_f32(sk, reinterpret_cast<float*>(loc + (size_t)b * nvls_region_), T, H, stream, &sg), op.nvls_part);
+                cuda_check(launch_ar_nvls_resid_rmsnorm(comm->nvls_multicast(), loc, (size_t)b * nvls_region_, (size_t)(2 + b) * nvls_region_, 4 * nvls_region_ + (size_t)b * 512, tp, tp_rank,
+                                                        x_, gain, xn_.x, T, H, cfg.rms_eps, stream, sg), op.nvls_ar);
+                MARK(7);
                 return;
             }
-            cuda_check(launch_gemm_streamk(a.map(), w.map(sk.bn), T, H, K, pf, stream, a.w8(w)), lb.gemm); MARK(mark);
-            if (use_tp) {      // row-parallel projection: all-reduce the rank partials over NVLink peer memory, then residual + norm
-                const int b = comm->next_buffer();
-                const TpComm::Signal sg = comm->next_signal();     // "buffer written" handshake rides on the two kernels: no barrier launch
-                if (comm->nvls() && T <= 128) {
-                    char* loc = reinterpret_cast<char*>(comm->nvls_local());
-                    cuda_check(launch_sk_reduce_f32(sk, reinterpret_cast<float*>(loc + (size_t)b * nvls_region_), T, H, stream, &sg), lb.nvls_part);
-                    cuda_check(launch_ar_nvls_resid_rmsnorm(comm->nvls_multicast(), loc, (size_t)b * nvls_region_, (size_t)(2 + b) * nvls_region_, 4 * nvls_region_ + (size_t)b * 512, tp, tp_rank,
-                                                            x_, gain, xn_.x, T, H, cfg.rms_eps, stream, sg), lb.nvls_ar);
-                } else if (opt.tp_ar_bf16) {
-                    cuda_check(launch_sk_reduce_bf16(sk, comm->sym(b), T, H, stream, &sg), lb.bf16_part);
-                    cuda_check(launch_ar_resid_rmsnorm_bf16in(comm->d_peer_sym(b), tp, x_, gain, xn_.x, T, H, cfg.rms_eps, stream, &sg), lb.ar);
-                } else {
-                    cuda_check(launch_sk_reduce_f32(sk, reinterpret_cast<float*>(comm->sym(b)), T, H, stream, &sg), lb.f32_part);
-                    cuda_check(launch_ar_resid_rmsnorm(comm->d_peer_sym(b), tp, x_, gain, xn_.x, T, H, cfg.rms_eps, stream, &sg), lb.ar);
-                }
-            } else {
-                cuda_check(launch_sk_resid_rmsnorm(sk, x_, gain, xn_.x, T, H, cfg.rms_eps, stream), lb.resid);
-            }
-            MARK(7);
+            tp_row_parallel_partial(g, opt.tp_ar_bf16, comm->sym(b), sg, op, stream, mark);
+            tp_row_parallel_finish(comm->d_peer_sym(b), tp, opt.tp_ar_bf16, x_, gain, xn_.x, T, H, cfg.rms_eps, sg, op, stream, mark);
         };
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
             quant(xn_);
-            if (ck_qkv) {
-                cuda_check(launch_gemm_clusterk_rope(&xn_.tm, ly.qkv.map(128), T, qkvd, H, ck_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh), stream),
-                           "qkv gemm + RoPE + KV write (cluster split-K)"); MARK(2);
-            } else if (fuse_rope) {
-                cuda_check(launch_gemm_streamk_rope(xn_.map(), ly.qkv.map(128), T, qkvd, H, pf_qkv, make_sk_rope_args(ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh),
-                                                    tile_flags_ + 0 * SK_MAX_FLAG_TILES, stream, xn_.w8(ly.qkv)), "qkv gemm + RoPE + KV write (stream-K)"); MARK(2);
-            } else {
-                cuda_check(launch_gemm_streamk(xn_.map(), ly.qkv.map(sk_qkv.bn), T, qkvd, H, pf_qkv, stream, xn_.w8(ly.qkv)), "qkv gemm (stream-K)"); MARK(2);
-                cuda_check(launch_sk_rope_kv_write(sk_qkv, ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope (stream-K)"); MARK(3);
-            }
+            qkv_rope(proj(path_qkv, xn_, ly.qkv, sk_qkv, 0), ly.bqkv, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, nh, stream, mark);
             attention(l);
             quant(attn_);
-            row_parallel(attn_, ly.o, qd, ck_o, fuse_o, sk_o, pf_o, 1, ly.ln2, 6, kOLabels);
+            row_parallel(attn_, ly.o, path_o, sk_o, 1, ly.ln2, kOProj);
             quant(xn_);
-            if (fuse_swiglu) {
-                cuda_check(launch_gemm_streamk_swiglu(&xn_.tm, ly.gu.map(128), T, F, H, pf_gu, act_.x, tile_flags_ + 2 * SK_MAX_FLAG_TILES, stream), "gate_up gemm + SwiGLU (stream-K)"); MARK(8);
-            } else {
-                cuda_check(launch_gemm_streamk(xn_.map(), ly.gu.map(sk_gu.bn), T, 2 * F, H, pf_gu, stream, xn_.w8(ly.gu)), "gate_up gemm (stream-K)"); MARK(8);
-                cuda_check(launch_sk_swiglu(sk_gu, act_.x, T, F, stream), "swiglu"); MARK(9);
-            }
+            gate_up_swiglu(proj(path_gu, xn_, ly.gu, sk_gu, 2), act_.x, stream, mark);
             quant(act_);
-            row_parallel(act_, ly.down, F, ck_dn, fuse_dn, sk_dn, pf_dn, 3, (l + 1 < L) ? layers[l + 1].ln1 : final_norm, 10, kDownLabels);
+            row_parallel(act_, ly.down, path_dn, sk_dn, 3, (l + 1 < L) ? layers[l + 1].ln1 : final_norm, kDownProj);
         }
     } else {
         // row-parallel projection (o, down) into x.  Single GPU: the residual add in the epilogue.  Tensor parallel: bf16 partial -> symmetric
         // buffer, barrier, x += sum over ranks (rank order)
-        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int K, int bn, int mark, const char* label) {
-            GemmParams g{}; g.M = T; g.N = H; g.K = K; g.ldo = H;
+        auto row_parallel = [&](const ProjInput& a, const WeightMat& w, int K, int bn, int mark_id, const char* label) {
             if (!use_tp) {
-                g.out = x_; g.resid = x_; g.ldr = H; g.w8 = a.w8(w);
-                cuda_check(launch_gemm(a.map(), w.map(bn), g, EPI_RESID, bn, stream), label); MARK(mark);
+                proj_gemm(a.map(), w.map(bn), T, H, K, EPI_RESID, bn, x_, nullptr, x_, a.w8(w), label, stream); MARK(mark_id);
                 return;
             }
             const int b = comm->next_buffer();
-            g.out = comm->sym(b);
-            cuda_check(launch_gemm(&a.tm, w.map(bn), g, EPI_STORE, bn, stream), label); MARK(mark);
+            proj_gemm(a.map(), w.map(bn), T, H, K, EPI_STORE, bn, comm->sym(b), nullptr, nullptr, a.w8(w), label, stream); MARK(mark_id);
             cuda_check(comm->barrier(stream), "xgpu barrier");
             if (T >= opt.tp_two_shot_rows) {
                 cuda_check(launch_ar2_reduce_scatter(comm->d_peer_sym(b), tp, tp_rank, x_, comm->sym(TpComm::GATHER), T, H, stream), "reduce-scatter+resid");
@@ -587,16 +543,14 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
             const Layer& ly = layers[l];
             cuda_check(launch_rmsnorm(x_, ly.ln1, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm1"); MARK(1);
             quant(xn_);
-            GemmParams g{}; g.M = T; g.N = qkvd; g.K = H; g.out = qkv_; g.ldo = qkvd; g.bias = ly.bqkv; g.w8 = xn_.w8(ly.qkv);
-            cuda_check(launch_gemm(xn_.map(), ly.qkv.map(bn_qkv), g, EPI_STORE, bn_qkv, stream), "qkv gemm"); MARK(2);
+            proj_gemm(xn_.map(), ly.qkv.map(bn_qkv), T, qkvd, H, EPI_STORE, bn_qkv, qkv_, ly.bqkv, nullptr, xn_.w8(ly.qkv), "qkv gemm", stream); MARK(2);
             cuda_check(launch_rope_kv_write(qkv_, d_pos, d_slot, rope_cos, rope_sin, q_, kv, l, T, nh, stream), "rope"); MARK(3);
             attention(l);
             quant(attn_);
             row_parallel(attn_, ly.o, qd, bn_o, 6, "o gemm");
             cuda_check(launch_rmsnorm(x_, ly.ln2, xn_.x, T, H, cfg.rms_eps, stream), "rmsnorm2"); MARK(1);
             quant(xn_);
-            GemmParams gg{}; gg.M = T; gg.N = 2 * F; gg.K = H; gg.out = act_.x; gg.ldo = F; gg.w8 = xn_.w8(ly.gu);
-            cuda_check(launch_gemm(xn_.map(), ly.gu.map(bn_gu), gg, EPI_SWIGLU, bn_gu, stream), "gate_up gemm"); MARK(8);
+            proj_gemm(xn_.map(), ly.gu.map(bn_gu), T, 2 * F, H, EPI_SWIGLU, bn_gu, act_.x, nullptr, nullptr, xn_.w8(ly.gu), "gate_up gemm", stream); MARK(8);
             quant(act_);
             row_parallel(act_, ly.down, F, bn_down, 10, "down gemm");
         }
@@ -610,23 +564,21 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
         }
         MARK(11);
         const int bn_lm = pick_bn(S, V, sm_count, opt.bn_lm);
-        const int n_tiles = gemm_n_tiles(V, bn_lm);
-        GemmParams gl{}; gl.M = S; gl.N = V; gl.K = H; gl.logits = logits_out; gl.ldl = V; gl.amax_val = amax_val_; gl.amax_idx = amax_idx_;
-        if (!in.mask_slots.empty()) {          // constrained rows: the arg-max runs over their state's allowed tokens, on every vocabulary shard
-            gl.mask_table = mask_table_; gl.mask_slot = d_meta_ + o_mslot; gl.mask_words = mask_words; gl.col_offset = tp_rank * V;
-        }
+        // constrained rows: the arg-max runs over their state's allowed tokens, on every vocabulary shard
+        const bool masked = !in.mask_slots.empty();
+        float* logits = logits_out;
         int lb = -1;
         if (use_tp) {          // vocab-parallel head: each rank's fp32 logits shard is staged in its symmetric buffer when asked for
-            gl.logits = nullptr;
+            logits = nullptr;
             if (in.want_logits) {
                 if ((size_t)S * V * 4 > comm->sym_bytes()) throw std::runtime_error("debug logits do not fit the symmetric buffer");
-                lb = comm->next_buffer(); gl.logits = reinterpret_cast<float*>(comm->sym(lb)); gl.ldl = V;
+                lb = comm->next_buffer(); logits = reinterpret_cast<float*>(comm->sym(lb));
             }
         }
-        cuda_check(launch_gemm(&tm_xsn_, lm_head.map(bn_lm), gl, EPI_LOGITS, bn_lm, stream), "lm_head gemm"); MARK(12);
+        const int b = use_tp ? comm->next_buffer() : 0;
+        lm_head_argmax(&tm_xsn_, lm_head.map(bn_lm), S, V, H, bn_lm, logits, V, amax_val_, amax_idx_, masked ? mask_table_ : nullptr,
+                       masked ? d_meta_ + o_mslot : nullptr, masked ? mask_words : 0, tp_rank * V, d_out_ids_, use_tp ? comm->arg(b) : nullptr, stream, mark);
         if (use_tp) {
-            const int b = comm->next_buffer();
-            cuda_check(launch_argmax_reduce_pair(amax_val_, amax_idx_, S, n_tiles, tp_rank * V, comm->arg(b), stream), "argmax (local shard)");
             cuda_check(comm->barrier(stream), "xgpu barrier");
             cuda_check(launch_ar_argmax(comm->d_peer_arg(b), tp, S, d_out_ids_, stream), "argmax (all ranks)");
             if (lb >= 0 && logits_out) {   // leader assembles the full [S, vocab] logits from the peers' shards over NVLink
@@ -635,8 +587,6 @@ void DeviceModel::forward(const StepInput& in, float* logits_out) {
                                                  cudaMemcpyDeviceToDevice, stream), "logits gather");
             }
             if (lb >= 0) cuda_check(comm->barrier(stream), "xgpu barrier");     // peers must not reuse the staged shard before the leader has read it
-        } else {
-            cuda_check(launch_argmax_reduce(amax_val_, amax_idx_, S, n_tiles, d_out_ids_, nullptr, stream), "argmax");
         }
         cuda_check(cudaMemcpyAsync(h_out_ids, d_out_ids_, (size_t)S * 4, cudaMemcpyDeviceToHost, stream), "ids D2H"); MARK(13);
         d2h_bytes += (size_t)S * 4;

@@ -7,6 +7,7 @@
 
 #include "config.hpp"
 #include "kernels.hpp"
+#include "stages.hpp"
 #include "tp_comm.hpp"
 
 namespace oa {
@@ -119,7 +120,5 @@ private:
     int max_rows_ = 0, max_sample_ = 0;
     DecodePlan plan_; std::vector<int32_t> zero_counters_; std::vector<PrefillTile> sorted_tiles_;
 };
-
-void cuda_check(cudaError_t e, const char* what);
 
 }  // namespace oa
