@@ -129,6 +129,11 @@ OA_API int oa_debug_prefill_logits(oa_engine*, const int32_t* tokens, int32_t n,
  * out[6]=sum of per-step device durations / steps (host gaps excluded); with n_out >= 8 + batch, out[8 + b] = the token id sequence b
  * sampled in the last timed step; with n_out >= 8 + 2 * batch (single GPU), out[8 + batch + b] = that token's fp32 logit */
 OA_API int oa_bench_decode(oa_engine*, int32_t batch, int32_t ctx_len, int32_t steps, int32_t warmup, double* out, int32_t n_out);
+/* The same synthetic workload as oa_bench_decode (same tokens, pages and step inputs, no warmup steps, single GPU), untimed: the fp32
+ * logits of every decode step -> logits_out[steps, batch, vocab] and the sampled ids -> ids_out[steps, batch].  mixed_rows > 0: the last
+ * step also carries a mixed_rows-token prefill chunk of one extra sequence (a mixed step: decode attention for the batch, prefill
+ * attention for the chunk); its row is not sampled. */
+OA_API int oa_debug_decode_logits(oa_engine*, int32_t batch, int32_t ctx_len, int32_t steps, int32_t mixed_rows, float* logits_out, int32_t* ids_out);
 
 /* in-situ per-kernel-class timings accumulated while OA_PROFILE_ALL=1 (JSON name -> [total ms, launches]) */
 OA_API int oa_debug_kernel_times(oa_engine*, char* buf, size_t n, int32_t reset);

@@ -39,7 +39,7 @@ SYMBOLS = [
     "oa_k_quant_rows_e4m3", "oa_k_gemm_fp8", "oa_k_gemm_streamk_fp8",
     "oa_k_sk_row_parallel", "oa_k_sk_swiglu", "oa_k_sk_qkv_rope", "oa_k_kv_write", "oa_k_decode_attention", "oa_k_gemm_logits_masked",
     "oa_k_prefill_gemm", "oa_k_step_attention", "oa_k_embed_gather", "oa_host_pick_bn",
-    "oa_k_tp_row_parallel", "oa_k_tp_allreduce_prefill", "oa_k_tp_lm_head_argmax",
+    "oa_k_tp_row_parallel", "oa_k_tp_allreduce_prefill", "oa_k_tp_lm_head_argmax", "oa_debug_decode_logits",
 ]
 
 _lib = None
@@ -72,6 +72,7 @@ def load() -> C.CDLL:
     L.oa_model_info.argtypes = [vp, C.c_char_p, C.c_size_t]; L.oa_model_info.restype = C.c_int
     L.oa_debug_prefill_logits.argtypes = [vp, vp, i32, vp]; L.oa_debug_prefill_logits.restype = C.c_int
     L.oa_bench_decode.argtypes = [vp, i32, i32, i32, i32, C.POINTER(C.c_double), i32]; L.oa_bench_decode.restype = C.c_int
+    L.oa_debug_decode_logits.argtypes = [vp, i32, i32, i32, i32, vp, vp]; L.oa_debug_decode_logits.restype = C.c_int
     L.oa_k_rmsnorm.argtypes = [vp, vp, vp, i32, i32, f32, vp]; L.oa_k_rmsnorm.restype = C.c_int
     L.oa_k_gemm.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]; L.oa_k_gemm.restype = C.c_int
     L.oa_k_gemm_streamk.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp]; L.oa_k_gemm_streamk.restype = C.c_int

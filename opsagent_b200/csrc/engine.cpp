@@ -182,82 +182,88 @@ public:
         return OA_OK;
     }
 
+    // The fp32 logits and sampled ids of every decode step of bench_decode's workload (see oa_debug_decode_logits): the forward's launch
+    // chain at any geometry, with the step inputs the benchmark times
+    int debug_decode_logits(int batch, int ctx_len, int steps, int mixed_rows, float* logits_out, int32_t* ids_out) {
+        const int n_seqs = batch + (mixed_rows > 0 ? 1 : 0);
+        if (opt_.tp != 1) return fail(OA_ERR_BAD_REQUEST, "debug decode logits: single GPU only");
+        if (batch <= 0 || n_seqs > opt_.max_batch || ctx_len <= 0 || steps <= 0 || ctx_len + steps + 1 > opt_.max_seq_len || mixed_rows < 0 ||
+            mixed_rows + 1 > opt_.max_seq_len || batch + mixed_rows > std::max(opt_.max_step_tokens, opt_.max_batch))
+            return fail(OA_ERR_BAD_REQUEST, "debug decode logits: batch (+1 with a mixed chunk) <= max_batch, ctx_len+steps < max_seq_len, batch+mixed_rows <= max_step_tokens");
+        std::lock_guard<std::mutex> step(step_mu_);
+        CallerDevice on_engine_device(opt_.device);
+        std::vector<std::vector<int32_t>> pages;
+        std::vector<int32_t> chunk_pages;
+        float* d_logits = nullptr;
+        int rc = OA_OK;
+        try {
+            const int V = model_.cfg.vocab;
+            if ((rc = alloc_synthetic_pages(batch, ctx_len + steps, pages)) != OA_OK) return rc;
+            {
+                std::lock_guard<std::mutex> lk(mu_);
+                if (mixed_rows > 0 && !alloc_pages_locked(chunk_pages, (mixed_rows + 63) / 64)) rc = fail(OA_ERR_OVERLOADED, "debug decode logits: not enough KV pages");
+            }
+            if (rc == OA_OK) {
+                cuda_check(cudaMalloc(&d_logits, (size_t)batch * V * 4), "cudaMalloc logits");
+                auto before = [&](int it, StepInput& in) {
+                    in.want_logits = true;
+                    if (it + 1 == steps && mixed_rows > 0) {      // mixed step: the batch's decode rows, then one new sequence's prefill chunk
+                        in.decode = false; in.n_decode = batch;
+                        const int sidx = in.n_seqs++, row0 = (int)in.tokens.size();
+                        in.block_tables.resize((size_t)in.n_seqs * model_.max_pages_per_seq, 0);
+                        for (size_t i = 0; i < chunk_pages.size(); ++i) in.block_tables[(size_t)sidx * model_.max_pages_per_seq + i] = chunk_pages[i];
+                        in.ctx_lens.push_back(mixed_rows);
+                        for (int i = 0; i < mixed_rows; ++i) {
+                            in.tokens.push_back(synth_token(batch, i, V)); in.positions.push_back(i); in.slots.push_back(chunk_pages[i / 64] * 64 + i % 64);
+                        }
+                        append_prefill_tiles(in.tiles, sidx, row0, 0, mixed_rows);
+                    }
+                    return d_logits;
+                };
+                auto after_sync = [&](int it) {
+                    cuda_check(cudaMemcpy(logits_out + (size_t)it * batch * V, d_logits, (size_t)batch * V * 4, cudaMemcpyDeviceToHost), "logits D2H");
+                    std::memcpy(ids_out + (size_t)it * batch, model_.h_out_ids, (size_t)batch * 4);
+                };
+                drive_synthetic_decode(pages, ctx_len, steps, [] {}, before, [](int) {}, after_sync);
+            }
+        } catch (const std::exception& ex) { rc = fail(OA_ERR_INTERNAL, ex.what()); }
+        if (d_logits) cudaFree(d_logits);
+        { std::lock_guard<std::mutex> lk(mu_); for (auto& pv : pages) for (int p : pv) release_page_locked(p); for (int p : chunk_pages) release_page_locked(p); }
+        return rc;
+    }
+
     int bench_decode(int batch, int ctx_len, int steps, int warmup, double* out, int n_out) {
         if (batch <= 0 || batch > opt_.max_batch || ctx_len <= 0 || ctx_len + steps + warmup + 1 > opt_.max_seq_len || n_out < 6)
             return fail(OA_ERR_BAD_REQUEST, "bench_decode: batch <= max_batch, ctx_len+steps+warmup < max_seq_len, n_out >= 6");
         std::lock_guard<std::mutex> step(step_mu_);
         CallerDevice on_engine_device(opt_.device);
         try {
-            const int V = model_.cfg.vocab;
-            const int total_len = ctx_len + steps + warmup;
-            const int pages_per = (total_len + 63) / 64;
-            std::vector<std::vector<int32_t>> pages(batch);
-            {
-                std::lock_guard<std::mutex> lk(mu_);
-                if ((long long)pages_per * batch > (long long)available_pages_locked()) return fail(OA_ERR_OVERLOADED, "bench_decode: not enough KV pages");
-                for (int b = 0; b < batch; ++b) alloc_pages_locked(pages[b], pages_per);
-            }
-            auto synth = [&](int b, int i) { uint64_t h = (uint64_t)(b + 1) * 0x9E3779B97F4A7C15ull + (uint64_t)i * 0xBF58476D1CE4E5B9ull; h ^= h >> 29; return (int32_t)(h % (uint64_t)V); };
+            std::vector<std::vector<int32_t>> pages;
+            if (int rc = alloc_synthetic_pages(batch, ctx_len + steps + warmup, pages)) return rc;
             cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
             const bool prof_all = model_.profile_all; model_.profile_all = false;      // in-situ kernel timing covers the decode steps only
-            // ---- prefill: ctx_len-1 tokens per sequence, chunked by the step token budget ----
-            const int P = ctx_len - 1;
-            cudaEventRecord(e0, model_.stream);
-            {
-                int b = 0, off = 0, n_fwd = 0;
-                const bool prof_prefill = std::getenv("OA_CUDA_PROFILER_PREFILL") != nullptr;
-                const bool skip_prefill = std::getenv("OA_BENCH_SKIP_PREFILL") != nullptr;   // dev profiling only: decode over whatever the (zero-initialised) pages hold
-                while (b < batch && P > 0 && !skip_prefill) {
-                    StepInput in; in.decode = false;
-                    int budget = opt_.max_step_tokens;
-                    while (b < batch && budget > 0 && in.n_seqs < opt_.max_batch) {
-                        const int take = std::min(budget, P - off);
-                        const int sidx = in.n_seqs++;
-                        in.block_tables.resize((size_t)in.n_seqs * model_.max_pages_per_seq, 0);
-                        for (size_t i = 0; i < pages[b].size(); ++i) in.block_tables[(size_t)sidx * model_.max_pages_per_seq + i] = pages[b][i];
-                        in.ctx_lens.push_back(off + take);
-                        const int row0 = (int)in.tokens.size();
-                        for (int i = off; i < off + take; ++i) { in.tokens.push_back(synth(b, i)); in.positions.push_back(i); in.slots.push_back(pages[b][i / 64] * 64 + i % 64); }
-                        append_prefill_tiles(in.tiles, sidx, row0, off, take);
-                        budget -= take; off += take;
-                        if (off >= P) { off = 0; ++b; }
-                    }
-                    if (prof_prefill && n_fwd == 1) { model_.sync(); cudaProfilerStart(); }     // the 2nd prefill chunk (warm)
-                    run_forward(in, nullptr);
-                    if (prof_prefill && n_fwd == 1) { model_.sync(); cudaProfilerStop(); }
-                    ++n_fwd;
-                }
-            }
-            cudaEventRecord(e1, model_.stream); model_.sync();
-            float prefill_ms = 0; cudaEventElapsedTime(&prefill_ms, e0, e1);
-            // ---- decode steps ----
-            model_.profile_all = prof_all;
-            std::vector<int32_t> last(batch);
-            for (int b = 0; b < batch; ++b) last[b] = synth(b, P);
+            float prefill_ms = 0;
             double ctx_sum = 0; float total_ms = 0; uint64_t launches0 = 0;
             cudaEvent_t eb0, eb1; cudaEventCreate(&eb0); cudaEventCreate(&eb1);
-            model_.attn_ms_accum = 0;
-            for (int it = 0; it < warmup + steps; ++it) {
-                const int pos = P + it;
-                StepInput in; in.decode = true; in.n_seqs = batch;
-                in.block_tables.assign((size_t)batch * model_.max_pages_per_seq, 0);
-                for (int b = 0; b < batch; ++b) {
-                    for (size_t i = 0; i < pages[b].size(); ++i) in.block_tables[(size_t)b * model_.max_pages_per_seq + i] = pages[b][i];
-                    in.tokens.push_back(last[b]); in.positions.push_back(pos); in.slots.push_back(pages[b][pos / 64] * 64 + pos % 64);
-                    in.ctx_lens.push_back(pos + 1); in.sample_rows.push_back(b);
-                }
+            cudaEventRecord(e0, model_.stream);
+            auto prefilled = [&] {
+                cudaEventRecord(e1, model_.stream); model_.sync();
+                cudaEventElapsedTime(&prefill_ms, e0, e1);
+                model_.profile_all = prof_all;
+                model_.attn_ms_accum = 0;
+            };
+            const int P = ctx_len - 1;
+            auto before = [&](int it, StepInput&) -> float* {
                 if (it == warmup) {
                     if (std::getenv("OA_CUDA_PROFILER")) { model_.sync(); cudaProfilerStart(); }   // ncu --profile-from-start off
                     launches0 = launches_total(); model_.attn_ms_accum = 0; cudaEventRecord(eb0, model_.stream);
                 }
-                const bool timed = it >= warmup;
-                if (timed) { cudaEventRecord(e0, model_.stream); ctx_sum += pos + 1; }
-                run_forward(in, nullptr);
-                if (timed) cudaEventRecord(e1, model_.stream);
-                model_.sync();
-                if (timed) { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); total_ms += ms; }
-                for (int b = 0; b < batch; ++b) last[b] = model_.h_out_ids[b];
-            }
+                if (it >= warmup) { cudaEventRecord(e0, model_.stream); ctx_sum += P + it + 1; }
+                return nullptr;
+            };
+            auto after_launch = [&](int it) { if (it >= warmup) cudaEventRecord(e1, model_.stream); };
+            auto after_sync = [&](int it) { if (it >= warmup) { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); total_ms += ms; } };
+            const std::vector<int32_t> last = drive_synthetic_decode(pages, ctx_len, warmup + steps, prefilled, before, after_launch, after_sync);
             cudaEventRecord(eb1, model_.stream); model_.sync();
             if (std::getenv("OA_CUDA_PROFILER")) cudaProfilerStop();
             float bracket_ms = 0; cudaEventElapsedTime(&bracket_ms, eb0, eb1);
@@ -331,6 +337,74 @@ private:
     void run_forward(const StepInput& in, float* logits_out) {
         if (model_.comm && opt_.tp_rank == 0) model_.comm->publish(in);
         model_.forward(in, logits_out);
+    }
+    // ---- the synthetic decode workload of bench_decode and debug_decode_logits ----
+    // seeded token i of synthetic sequence b
+    static int32_t synth_token(int b, int i, int V) {
+        uint64_t h = (uint64_t)(b + 1) * 0x9E3779B97F4A7C15ull + (uint64_t)i * 0xBF58476D1CE4E5B9ull; h ^= h >> 29; return (int32_t)(h % (uint64_t)V);
+    }
+    // pages for `batch` sequences of total_len tokens each, or OA_ERR_OVERLOADED with nothing taken
+    int alloc_synthetic_pages(int batch, int total_len, std::vector<std::vector<int32_t>>& pages) {
+        const int pages_per = (total_len + 63) / 64;
+        pages.assign(batch, {});
+        std::lock_guard<std::mutex> lk(mu_);
+        if ((long long)pages_per * batch > (long long)available_pages_locked()) { pages.clear(); return fail(OA_ERR_OVERLOADED, "synthetic decode batch: not enough KV pages"); }
+        for (int b = 0; b < batch; ++b) alloc_pages_locked(pages[b], pages_per);
+        return OA_OK;
+    }
+    // Prefills ctx_len - 1 synthetic tokens of each sequence in pages[b], several sequences per forward, chunked by the step token budget;
+    // then runs n_steps decode steps of the whole batch, each feeding back the ids the previous one sampled.  Hooks: prefilled() once the
+    // prefill is enqueued; per decode step, before(it, in) may amend the step input and returns the device logits buffer of the forward (or
+    // null), after_launch(it) runs once the step is enqueued and after_sync(it) once it has completed.  Returns the ids of the last step.
+    template <class Prefilled, class Before, class AfterLaunch, class AfterSync>
+    std::vector<int32_t> drive_synthetic_decode(const std::vector<std::vector<int32_t>>& pages, int ctx_len, int n_steps, Prefilled&& prefilled,
+                                                Before&& before, AfterLaunch&& after_launch, AfterSync&& after_sync) {
+        const int V = model_.cfg.vocab, batch = (int)pages.size(), P = ctx_len - 1;
+        {
+            int b = 0, off = 0, n_fwd = 0;
+            const bool prof_prefill = std::getenv("OA_CUDA_PROFILER_PREFILL") != nullptr;
+            const bool skip_prefill = std::getenv("OA_BENCH_SKIP_PREFILL") != nullptr;   // dev profiling only: decode over whatever the (zero-initialised) pages hold
+            while (b < batch && P > 0 && !skip_prefill) {
+                StepInput in; in.decode = false;
+                int budget = opt_.max_step_tokens;
+                while (b < batch && budget > 0 && in.n_seqs < opt_.max_batch) {
+                    const int take = std::min(budget, P - off);
+                    const int sidx = in.n_seqs++;
+                    in.block_tables.resize((size_t)in.n_seqs * model_.max_pages_per_seq, 0);
+                    for (size_t i = 0; i < pages[b].size(); ++i) in.block_tables[(size_t)sidx * model_.max_pages_per_seq + i] = pages[b][i];
+                    in.ctx_lens.push_back(off + take);
+                    const int row0 = (int)in.tokens.size();
+                    for (int i = off; i < off + take; ++i) { in.tokens.push_back(synth_token(b, i, V)); in.positions.push_back(i); in.slots.push_back(pages[b][i / 64] * 64 + i % 64); }
+                    append_prefill_tiles(in.tiles, sidx, row0, off, take);
+                    budget -= take; off += take;
+                    if (off >= P) { off = 0; ++b; }
+                }
+                if (prof_prefill && n_fwd == 1) { model_.sync(); cudaProfilerStart(); }     // the 2nd prefill chunk (warm)
+                run_forward(in, nullptr);
+                if (prof_prefill && n_fwd == 1) { model_.sync(); cudaProfilerStop(); }
+                ++n_fwd;
+            }
+        }
+        prefilled();
+        std::vector<int32_t> last(batch);
+        for (int b = 0; b < batch; ++b) last[b] = synth_token(b, P, V);
+        for (int it = 0; it < n_steps; ++it) {
+            const int pos = P + it;
+            StepInput in; in.decode = true; in.n_seqs = batch;
+            in.block_tables.assign((size_t)batch * model_.max_pages_per_seq, 0);
+            for (int b = 0; b < batch; ++b) {
+                for (size_t i = 0; i < pages[b].size(); ++i) in.block_tables[(size_t)b * model_.max_pages_per_seq + i] = pages[b][i];
+                in.tokens.push_back(last[b]); in.positions.push_back(pos); in.slots.push_back(pages[b][pos / 64] * 64 + pos % 64);
+                in.ctx_lens.push_back(pos + 1); in.sample_rows.push_back(b);
+            }
+            float* logits = before(it, in);
+            run_forward(in, logits);
+            after_launch(it);
+            model_.sync();
+            after_sync(it);
+            for (int b = 0; b < batch; ++b) last[b] = model_.h_out_ids[b];
+        }
+        return last;
     }
     void follow() {
         cudaSetDevice(opt_.device);
@@ -795,6 +869,10 @@ int oa_bench_decode(oa_engine* h, int32_t batch, int32_t ctx_len, int32_t steps,
     int rc = h->e->bench_decode(batch, ctx_len, steps, warmup, out, n_out);
     h->e->model().profile_attn = false; h->e->model().profile_all = false;
     return rc;
+}
+int oa_debug_decode_logits(oa_engine* h, int32_t batch, int32_t ctx_len, int32_t steps, int32_t mixed_rows, float* logits_out, int32_t* ids_out) {
+    if (!h || !logits_out || !ids_out) return fail(OA_ERR_BAD_REQUEST, "null argument");
+    return h->e->debug_decode_logits(batch, ctx_len, steps, mixed_rows, logits_out, ids_out);
 }
 int oa_debug_kernel_times(oa_engine* h, char* buf, size_t n, int32_t reset) {
     if (!h || !buf) return fail(OA_ERR_BAD_REQUEST, "null argument");

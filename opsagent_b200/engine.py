@@ -144,6 +144,15 @@ class Engine:
         _check(self._L.oa_debug_prefill_logits(self._h, toks.ctypes.data, len(toks), out.ctypes.data))
         return out
 
+    def debug_decode_logits(self, batch: int, ctx_len: int, steps: int, mixed_rows: int = 0):
+        """bench_decode's workload, untimed: -> (fp32 logits [steps, batch, vocab], sampled ids [steps, batch]); mixed_rows > 0 makes the
+        last step a mixed step that also prefills a mixed_rows-token chunk of one extra sequence"""
+        import numpy as np
+        logits = np.empty((steps, batch, self.info["vocab"]), dtype=np.float32)
+        ids = np.empty((steps, batch), dtype=np.int32)
+        _check(self._L.oa_debug_decode_logits(self._h, batch, ctx_len, steps, mixed_rows, logits.ctypes.data, ids.ctypes.data))
+        return logits, ids
+
     def kernel_times(self, reset: bool = True) -> dict:
         buf = C.create_string_buffer(4096)
         _check(self._L.oa_debug_kernel_times(self._h, buf, 4096, int(reset)))

@@ -7,6 +7,7 @@ noise floor of ~5e-2 between bf16-faithful and fp32 arithmetic):
     LOGIT_TOL  = 2.5e-2 absolute on fp32 logits, GPU vs oracle(bf16 mode)  — accumulation-order + exp2/expf effects
     token ids  : must be identical wherever the oracle's top1-top2 margin exceeds 2*LOGIT_TOL
 """
+import dataclasses
 import json
 import os
 import threading
@@ -348,7 +349,7 @@ def _bpe_template_ids(tokenizer_json, msgs):
     return ids + [sp["<|start_header_id|>"]] + enc("assistant") + [sp["<|end_header_id|>"]] + enc("\n\n")
 
 
-def _full_size_parity(name, prompt_msgs, n_new, kv_pages, tokenizer=None, logit_rows=None, floor=None):
+def _full_size_parity(name, prompt, n_new, kv_pages, tokenizer=None, logit_rows=None, floor=None, overrides=None):
     """At 16-80 layers the bf16 rounding of every stored activation makes two bf16 computations with different fp32 accumulation
     orders drift apart chaotically: the CPU oracle in bf16-faithful mode itself sits `floor` away from its own fp32 mode.  Stated
     tolerance at full size: the engine's fp32 logits must be as close to the oracle's fp32-activation logits as 1.5x that floor
@@ -356,18 +357,25 @@ def _full_size_parity(name, prompt_msgs, n_new, kv_pages, tokenizer=None, logit_
     tokenizer: a tokenizer.json (the prompt is then the reference's real text through a real BPE); logit_rows: prompt positions whose
     logits are compared (default: all).  floor = (max, mean) measured by an earlier call on the same model: the fp32-mode oracle pass is
     then skipped (a 1,536-token prompt costs minutes of CPU per pass) and the engine is compared with the bf16-faithful oracle directly,
-    within 2.5x the floor (triangle inequality: 1.5x to the fp32 oracle + 1x between the oracle's two modes)."""
-    spec = O.PRESETS[name]
-    cfg = {"model": name, "num_pages": kv_pages, "max_seq_len": 2048, "max_batch": 8, "max_step_tokens": 2048, "seed": spec.seed}
+    within 2.5x the floor (triangle inequality: 1.5x to the fp32 oracle + 1x between the oracle's two modes).
+    prompt: chat messages [(role, content)] (through the chat template) or the prompt's token ids.  overrides: preset fields replaced on both
+    sides (engine config and ModelSpec), e.g. fewer layers and random norm gains."""
+    overrides = overrides or {}
+    spec = dataclasses.replace(O.PRESETS[name], **overrides)
+    cfg = {"model": name, "num_pages": kv_pages, "max_seq_len": 2048, "max_batch": 8, "max_step_tokens": 2048, "seed": spec.seed, **overrides}
     if tokenizer:
         cfg["tokenizer"] = tokenizer
     eng = Engine(cfg)
-    ids = eng.apply_chat_template(prompt_msgs)
-    assert ids == (_bpe_template_ids(tokenizer, prompt_msgs) if tokenizer else O.apply_chat_template(spec, prompt_msgs))
+    chat = isinstance(prompt[0], tuple)
+    if chat:
+        ids = eng.apply_chat_template(prompt)
+        assert ids == (_bpe_template_ids(tokenizer, prompt) if tokenizer else O.apply_chat_template(spec, prompt))
+    else:
+        ids = [int(t) for t in prompt]
     toks = np.array(ids, np.int32)
     rows = list(range(len(ids))) if logit_rows is None else [r if r >= 0 else len(ids) + r for r in logit_rows]
     got = eng.debug_prefill_logits(ids)[rows]
-    out = eng.chat_complete(name, prompt_msgs, n_new, flags=1)
+    out = eng.chat_complete(name, prompt, n_new, flags=1) if chat else eng.generate(ids, n_new, flags=1)
     eng.close()
     assert np.isfinite(got).all()
     orc1 = O.Oracle(spec, max_pos=len(ids) + n_new + 8, mode=1)
@@ -435,6 +443,21 @@ def test_full_size_llama_3_8b_matches_oracle():
                             floor=(short["floor_max"], short["floor_mean"]))
     assert res["prompt_tokens"] == P
     print("llama-3-8b analyze:", res)
+
+
+@pytest.mark.parametrize("name", ["llama-3-8b", "qwen2.5-32b", "llama-3-70b"])
+def test_production_width_with_random_norm_gains_matches_oracle(name):
+    """The production widths through DeviceModel::forward on one GPU, two layers deep: Llama-3-8B, Qwen2.5-32B (qkv bias at H = 5120,
+    rope theta 1e6, eps 1e-6, untied 152,064-row head) and Llama-3-70B (H = 8192, 64 query heads).  Random norm gains (the presets have
+    gains of exactly 1): a gain applied in the wrong place — ln2 for ln1, the next layer's ln1 for the final norm — changes the logits.
+    Prompts of 1 and 37 tokens (one stream-K row tile), 128 (a full one) and 200 (the tile path); logits of every prompt row and 12 greedy
+    tokens, within the full-size floor rule of _full_size_parity."""
+    spec = O.PRESETS[name]
+    rng = np.random.default_rng(42)
+    for n in (1, 37, 128, 200):
+        toks = rng.integers(0, spec.vocab, size=n).astype(np.int32)
+        res = _full_size_parity(name, toks, 12, 64, overrides=dict(n_layers=2, norm_random=1))
+        print(f"{name} n_layers=2 norm_random=1 prompt {n}:", res)
 
 
 @pytest.mark.parametrize("front", ["native", "python"])
